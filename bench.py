@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the PPO hot path (BASELINE.json metric: env-steps/sec, PPO update included).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--epochs E] [--engine auto|simt|tcgen05]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--epochs E] [--engine auto|simt|tcgen05] [--dump-outputs DIR]
 
 One "step" = one full PPO iteration of BASELINE config 2 per GPU: 128 rollout steps of 4096 synthetic Box(376)/Box(17)
 envs (policy+critic forward, sampling, buffer writes), bootstrap values + GAE, then nr_epochs x (B / minibatch) shuffled
@@ -16,6 +16,8 @@ Prints ONE JSON line (rank 0).  Keys beyond the base contract:
   cpu_baseline  the CPU oracle (oracle/ppo_oracle.py, torch fp32 on all host cores) on a bounded sample of the same workload
   e2e           same metric through PPO.train()'s loop with a NUMPY-interface env: observations/rewards in pinned HOST memory,
                 H2D every step, actions D2H every step, metrics D2H every iteration
+`--dump-outputs DIR` writes what the last timed iteration computed (see dump_outputs) as DIR/<name>.npy, so that two builds can be
+compared output for output: every input is seeded, so the same arguments give the same inputs.
 `--impl reference` times the CPU oracle alone (the reference's algorithm restated with the same torch primitives; the
 reference itself is Python and does not travel to the GPU box).
 """
@@ -43,7 +45,7 @@ def measured_peaks():
     if os.path.exists(path):
         p = json.load(open(path))
         return dict(hbm_gbs=p["hbm_gbs"], tflops=p.get("bf16_tflops_sustained", p["bf16_tflops"]), source="measured (MEASURED_PEAKS.json, sustained bf16)")
-    return dict(hbm_gbs=6650.0, tflops=1400.0, source="fallback (B200_PROFILING.md)")
+    return dict(hbm_gbs=3350.0, tflops=989.0, source="fallback (H100 SXM data sheet: HBM3 bandwidth, dense bf16)")
 
 
 # ---------------------------------------------------------------------------------------------------- clocks sampler
@@ -149,6 +151,25 @@ def timed_iterations(model, steps, dist):
     if dist is not None:
         dist.barrier()
     return e0.elapsed_time(e1) / 1e3, t0, t1
+
+
+DUMP_SAMPLE_ROWS = 65536  # rollout rows (t, env) kept by --dump-outputs: a fixed seeded sample, ~7 MB in all
+
+
+def dump_outputs(model, out_dir):
+    """What one PPO iteration hands its caller, as float32 .npy files: the updated flat parameters and Adam moments, the per-minibatch
+    metric records, and a fixed seeded sample of the rollout's actions, log-probs, values, advantages and returns."""
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    b = model.batch
+    T, N = model.nr_steps, model.nr_envs
+    rows = np.sort(np.random.default_rng(0).choice(T * N, size=min(DUMP_SAMPLE_ROWS, T * N), replace=False))
+    sel = torch.from_numpy(rows).to(b.actions.device)
+    arrays = {"params": model.params.flat, "adam_exp_avg": model.exp_avg, "adam_exp_avg_sq": model.exp_avg_sq, "metrics": model.metrics_dev,
+              "actions": b.actions.reshape(T * N, -1)[sel], "log_probs": b.log_probs.reshape(-1)[sel], "values": b.values.reshape(-1)[sel],
+              "advantages": b.advantages.reshape(-1)[sel], "returns": b.returns.reshape(-1)[sel]}
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
 
 
 def available_cores():
@@ -390,9 +411,9 @@ _AUX_VERDICT = None
 
 
 def aux_paths_verdict():
-    """May the FastSAC / PPO+LSTM workloads use (1) the tcgen05 3xTF32 engine for their dense layers (rlx_set_aux_gemm_engine) and (2) the
-    one-launch-per-direction LSTM recurrence (rlx_set_lstm_persistent)?  Both switches were written after the round's GPU budget was spent,
-    so they have to prove themselves ON THIS BOX before a timed run may use them: a subprocess (a kernel that traps or faults takes its CUDA
+    """May the FastSAC / PPO+LSTM workloads use (1) the wgmma 3xTF32 engine for their dense layers (rlx_set_aux_gemm_engine) and (2) the
+    one-launch-per-direction LSTM recurrence (rlx_set_lstm_persistent)?  Both switches are off by default, so each run proves them on the
+    device it times before a timed run may use them: a subprocess (a kernel that traps or faults takes its CUDA
     context along - not this process's) runs, with the switches on, the FastSAC golden-batch parity test, the SIMT-vs-tensor gradient
     agreement at batch 1024, the PPO+LSTM oracle parity tests at the config-5 shape (T=128, 256 envs) and a smaller one, and the bit-for-bit
     comparison of the two recurrence paths.  Green AND the paths actually counted -> on.  If both together fail, each is tried alone.  The
@@ -459,7 +480,7 @@ def with_aux_paths(fn, args):
         line = fn(args)
     finally:
         after = switches(False, False)
-    line["gemm_engine"] = dict(verdict, engine="tcgen05-3xTF32" if verdict["tensor_engine"] else "simt", tensor_gemms_in_run=after[0] - before[0],
+    line["gemm_engine"] = dict(verdict, engine="wgmma-3xTF32" if verdict["tensor_engine"] else "simt", tensor_gemms_in_run=after[0] - before[0],
                                persistent_launches_in_run=after[1] - before[1])
     return line
 
@@ -650,7 +671,7 @@ def workload_config(args, world):
             "parallelism": (f"dp{world} (env-sharded, " + ("reference-exact global permutation" if args.exact_permutation else "rank-local PCG64 shuffles")
                             + (", 1 peer-memory all-reduce kernel (rlx_comm, NVLink loads) of the flat gradient per minibatch)" if args.exchange == "peer"
                                else ", 1 NCCL all-reduce of the flat gradient per minibatch)")) if world > 1 else "single GPU",
-            "l2_policy": "per-step working set (rollout buffer 0.83 GB + gathered copy 0.83 GB + activations) exceeds the 126 MB L2"}
+            "l2_policy": "per-step working set (rollout buffer 0.83 GB + gathered copy 0.83 GB + activations) exceeds the 50 MB L2"}
 
 
 def main():
@@ -670,7 +691,7 @@ def main():
     ap.add_argument("--head-engine", default="fused", choices=["fused", "gemm", "mma"],
                     help="PPO loss head: fused SIMT kernel, the GEMM formulation, or the fused mma.sync kernel")
     ap.add_argument("--workload", default="ppo", choices=["ppo", "sac", "fastsac", "ppo_lstm"])
-    ap.add_argument("--tc-pair", default="", help="tcgen05 CTA-pair engine: MODE[:FWD_BN], MODE 0 off / 1 weight gradients (default) / 2 all GEMMs, FWD_BN 128|256")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR", help="write the last timed iteration's outputs as DIR/<name>.npy")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-bf16", action="store_true", help="N=1: skip the bf16-autocast sub-line")
@@ -680,6 +701,8 @@ def main():
     ap.add_argument("--no-strict", action="store_true", help="N>1: skip the second timed region at the contract's GLOBAL minibatch of 32768")
     ap.add_argument("--global-minibatch", type=int, default=0, help="N>1: headline region with this GLOBAL minibatch instead of --minibatch per GPU")
     args = ap.parse_args()
+    if args.dump_outputs and (args.workload != "ppo" or args.impl == "reference"):
+        ap.error("--dump-outputs writes the PPO workload's outputs; it cannot be combined with --workload sac|fastsac|ppo_lstm or --impl reference")
     args.warmup = max(args.warmup, 3) if args.impl != "reference" else args.warmup
 
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
@@ -693,7 +716,7 @@ def main():
             print(json.dumps(fn(args) if args.workload == "sac" or args.no_aux_engine else with_aux_paths(fn, args)))
         return
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device (the B200 arm has no CPU fallback; use --impl reference for the CPU oracle)")
+        raise SystemExit("bench.py: no CUDA device (the GPU arm has no CPU fallback; use --impl reference for the CPU oracle)")
     torch.cuda.set_device(local_rank)
     dist = None
     if world > 1:
@@ -703,9 +726,6 @@ def main():
     from rl_x_b200 import _native as nt
     lib = nt.load()
     lib.rlx_set_head_engine({"fused": 0, "gemm": 1, "mma": 2}[args.head_engine])
-    if args.tc_pair:
-        mode, _, bn = args.tc_pair.partition(":")
-        lib.rlx_set_tc_pair(int(mode), int(bn or 0))
 
     # ---- multi-GPU parity, visible to whoever runs the bench: the env-sharded run (reference-exact global permutation, this exchange, this
     # GEMM engine) against the same global problem on ONE GPU (tests/dist_check_ppo.py: 64 envs x 16 steps, obs 376 / act 17 / hidden 256,
@@ -735,6 +755,8 @@ def main():
     lib.rlx_reset_launch_count()
     seconds, t0, t1 = timed_iterations(model, args.steps, dist)
     launches = int(lib.rlx_launch_count())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(model, args.dump_outputs)
     clocks = sampler.stop(t0, t1) if sampler else None
     if dist is not None:
         tt = torch.tensor([seconds], device="cuda")
@@ -750,7 +772,7 @@ def main():
     classes = nt.timing_end()
     kernel_ms = {k: round(v["ms"] / 2, 4) for k, v in classes.items() if v["launches"]}
     tc_shape_ok = C2["hidden"] % 128 == 0 and C2["obs_dim"] % 4 == 0
-    engine = "tcgen05-3xTF32" if lib.rlx_get_gemm_engine() == 1 and tc_shape_ok else "simt-fp32"
+    engine = "wgmma-3xTF32" if lib.rlx_get_gemm_engine() == 1 and tc_shape_ok else "simt-fp32"
     peaks = measured_peaks()
     gemm = {k: classes[k] for k in ("gemm_fwd", "gemm_dx", "gemm_dw")}
     gflops, gms = sum(v["flops"] for v in gemm.values()), sum(v["ms"] for v in gemm.values())
@@ -760,14 +782,6 @@ def main():
                 "unit": "TFLOP/s", "frac": achieved_tf / peaks["tflops"], "traffic": None, "peak_source": peaks["source"],
                 "share_of_step": gms / total_ms if total_ms else None,
                 "note": "fp32-equivalent algorithmic FLOPs (2*M*N*K) of the exact-fp32 path against the dense bf16 tensor peak"}
-    # DRAM traffic per GEMM launch from the committed ncu --set full capture (profiles/roofline_traffic.json), next to the algorithmic bytes
-    try:
-        with open(os.path.join(ROOT, "profiles", "roofline_traffic.json")) as fh:
-            tr = json.load(fh)
-        roofline["traffic"] = tr["gemm_dram_bytes_per_minibatch"] / tr["gemm_launches_per_minibatch"]
-        roofline["traffic_source"] = tr["note"]
-    except (OSError, KeyError, ValueError):
-        pass
     glaunch = sum(v["launches"] for v in gemm.values())
     roofline["algorithmic_bytes_per_launch"] = sum(v["bytes"] for v in gemm.values()) / glaunch if glaunch else None
     # what the tensor pipe actually executes: 3 TF32 MMAs per fp32 product, against the tf32 dense rate (half the measured bf16 rate)
@@ -891,7 +905,7 @@ def main():
             g16 = {k: cls16[k] for k in ("gemm_fwd", "gemm_dx", "gemm_dw")}
             tf16 = sum(v["flops"] for v in g16.values()) / (sum(v["ms"] for v in g16.values()) * 1e-3) / 1e12
             line["bf16_autocast"] = {"value": steps_per_iter * args.steps / sb, "unit": "env-steps/s", "ms_per_step": sb / args.steps * 1e3, "dtype": "bf16-autocast",
-                                     "note": "bf16_mixed_precision_training=True: bf16 values in fp32 storage, ONE tcgen05 kind::tf32 MMA per product (exact for bf16 operands), "
+                                     "note": "bf16_mixed_precision_training=True: bf16 values in fp32 storage, ONE tf32 wgmma per product (exact for bf16 operands), "
                                              "fp32 accumulation, losses / clipping / Adam in fp32 as in the reference",
                                      "kernel_ms": {k: round(v["ms"] / 2, 4) for k, v in cls16.items() if v["launches"]},
                                      "roofline": {"bound": "tensor", "achieved": tf16, "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": tf16 / peaks["tflops"],

@@ -1,5 +1,5 @@
 /*
- * rlx_b200.h — C-ABI of the B200-native (sm_100a) RL-X hot path.
+ * rlx_b200.h — C-ABI of the CUDA-native (H100, sm_90a) RL-X hot path.
  *
  * The reference (nico-bohlinger/RL-X) is pure Python and has no FFI of its own; its hot path is the body of
  * PPO.train() (rl_x/algorithms/ppo/pytorch/ppo.py:97-393) and SAC.train() (rl_x/algorithms/sac/pytorch/sac.py:89-348).
@@ -47,17 +47,17 @@ void rlx_add_launch_count(uint64_t n);        /* account for kernels replayed th
 int rlx_timing_begin(void);
 int rlx_timing_end(double* ms, uint64_t* launches, double* flops, double* bytes);
 const char* rlx_kernel_class_name(int cls);
-/* GEMM engine used by the MLP entry points: 0 = fp32 SIMT (FFMA), 1 = tcgen05 3xTF32 (tensor cores, TMEM accumulators).
+/* GEMM engine used by the MLP entry points: 0 = fp32 SIMT (FFMA), 1 = wgmma 3xTF32 (tensor cores, register accumulators).
  * Returns the engine actually in effect (a request for 1 falls back to 0 with an error string if the shape is unsupported). */
 int rlx_set_gemm_engine(int engine);
 int rlx_get_gemm_engine(void);
 /* The same choice for the dense layers of the FastSAC and PPO+LSTM entry points (their own switch: these paths were validated on the SIMT
- * engine).  1 routes every GEMM whose layout / epilogue / alignment the tcgen05 engine covers to it and leaves the rest on the SIMT
+ * engine).  1 routes every GEMM whose layout / epilogue / alignment the wgmma engine covers to it and leaves the rest on the SIMT
  * engine (e.g. the 101-column logits of the C51 critics, whose row pitch is not a multiple of 16 bytes).  Default 0.  Returns the value in effect. */
 int rlx_set_aux_gemm_engine(int engine);
-uint64_t rlx_aux_tc_gemm_count(void);     /* GEMMs of those two paths that ran on the tcgen05 engine since load */
+uint64_t rlx_aux_tc_gemm_count(void);     /* GEMMs of those two paths that ran on the wgmma engine since load */
 
-/* Test hook: one plain fp32 GEMM through either engine.  layout 0: C[M,N] = A[M,K] B[N,K]^T; 1: C = A[M,K] B[K,N];
+/* Test hook: one plain fp32 GEMM through either engine (0 = SIMT, 1 = wgmma; any other value is RLX_ERR_INVALID_ARG).  layout 0: C[M,N] = A[M,K] B[N,K]^T; 1: C = A[M,K] B[K,N];
  * 2: C = A[K,M]^T B[K,N].  epilogue 0 none, 1 tanh(x + bias[n]) (layout 0), 2 x * (1 - aux[m,n]^2) (layout 1). */
 int rlx_debug_gemm_f32(int engine, int layout, int epilogue, int64_t M, int64_t N, int64_t K, const float* A, int64_t lda,
                        const float* B, int64_t ldb, float* C, int64_t ldc, const float* bias, const float* aux, int64_t ldaux,
@@ -288,15 +288,11 @@ int rlx_set_head_engine(int engine);
  * holds in a bf16 tensor to bf16 where torch rounds it - Linear inputs, weights and biases, Linear outputs, tanh outputs, the sampled action
  * and the bf16 subtraction / square inside its log-prob, gamma * next_values, and on the way back the gradients of those bf16 tensors and the
  * weight / bias gradients (one rounding of the complete fp32-accumulated sum) - while storage, losses, clipping and Adam stay fp32 as in
- * the reference.  bf16 values are exact TF32 operands, so the tensor-core GEMMs run ONE kind::tf32 MMA per product in this mode (fp32
- * accumulation in TMEM, as a bf16 tensor-core GEMM accumulates) instead of the three of the fp32-equivalent split.  Returns the setting. */
+ * the reference.  bf16 values are exact TF32 operands, so the tensor-core GEMMs run ONE tf32 wgmma per product in this mode (fp32
+ * accumulation, as a bf16 tensor-core GEMM accumulates) instead of the three of the fp32-equivalent split.  Returns the setting. */
 int rlx_set_autocast_bf16(int on);
-/* tcgen05 engine on CTA pairs (cta_group::2, csrc/gemm_tc2.cu).  mode 0: single-CTA kernels only; 1: the weight-gradient GEMMs of the PPO
- * update run on pairs (256 x 256 / 256 x 192 tiles); 2 (default, with fwd_bn = 128): the forward / dX GEMMs too, with fwd_bn-wide pair tiles
- * (128: double-buffered accumulators, 256: single; other values keep the current setting).  Returns the mode. */
-int rlx_set_tc_pair(int mode, int fwd_bn);
 /* 1: rlx_ppo_update_epoch_f32 runs gradient assembly + both grad norms + clip + Adam of a minibatch as ONE kernel (grid barrier in the
- * caller's workspace); 0 (default; measured faster on B200): the three separate kernels of rlx_ppo_minibatch_fwdbwd_f32 /
+ * caller's workspace); 0 (default): the three separate kernels of rlx_ppo_minibatch_fwdbwd_f32 /
  * rlx_gradnorm_clip_adam_f32.  Returns the setting. */
 int rlx_set_fused_tail(int on);
 /* bring-up / test entry of the GEMM head on caller buffers: H2 [m, 2*hidden] (policy | critic halves), torch-layout head weights; outputs
@@ -311,8 +307,7 @@ int rlx_debug_ppo_head_gemm_f32(int64_t m, int32_t hidden, int32_t act_dim, cons
 /* SURVEY.md §8 a18: rl_x/algorithms/ppo_lstm/flax (policy.py:36-146, critic.py:18-30, ppo_lstm.py:107-231), including the two policy
  * options lstm_obs_combine_method = "concat" | "film" (policy.py:57-59, 99-105) and share_lstm_obs_encoder (policy.py:51-53, 120-123).
  * The sources also compile for the host (g++ -DRLX_EMU) and are checked there against oracle/ppo_lstm_oracle.py
- * (tests/test_lstm_emulation.py); the default options have run on B200 since round 1, FiLM / shared encoder and the one-launch-per-step
- * recurrence were added after the round-2 GPU budget was spent (emulation-validated; GPU tests in tests/test_gpu_zzz_ppo_lstm.py).
+ * (tests/test_lstm_emulation.py), all options included; the GPU tests are in tests/test_gpu_zzz_ppo_lstm.py.
  * Exact-fp32 SIMT GEMMs; ONE launch per time step for the recurrent part in both directions (carry reset + h.Wh + cell fused).
  *
  * Flat parameter layouts (fp32).  All kernels are stored [in, out] like Flax.  Policy segments, in order:
@@ -402,9 +397,9 @@ int rlx_optax_clip_adam_f32(float* params, const float* grads, float* mu, float*
 int rlx_gather_env_columns_f32(const float* src, const int64_t* env_idx, int64_t T, int64_t N, int64_t n, int64_t width, float* out, void* stream);
 
 /* -------------------------------------------------------------------------------------------- FastSAC update -- */
-/* SURVEY.md §8 f4 (second half): rl_x/algorithms/fastsac/pytorch, fp32 path.  STATUS: written
- * without GPU access; numerics checked by running these sources in a host emulation build against oracle/fastsac_oracle.py, which
- * is pinned to the executed reference (tests/test_fastsac_emulation.py); on hardware since the round-1 driver run (tests/test_gpu_zzzz_fastsac.py).
+/* SURVEY.md §8 f4 (second half): rl_x/algorithms/fastsac/pytorch, fp32 path.  Numerics are also checked by running these sources in a
+ * host emulation build against oracle/fastsac_oracle.py, which
+ * is pinned to the executed reference (tests/test_fastsac_emulation.py); GPU tests: tests/test_gpu_zzzz_fastsac.py.
  * Networks (fixed widths like the reference): policy Linear-LayerNorm-SiLU x3 (512, 256, 128) + mean / log_std heads (policy.py:36-48);
  * Q network Linear-LayerNorm-SiLU x3 (768, 384, 192) + nr_atoms logits on [state | action] (q_network.py:24-35).
  * Flat parameter layouts, torch [out, in] weights in state_dict order:

@@ -2,7 +2,7 @@
 """Per-kernel summary of an `ncu --set full` capture:  ncu -i X.ncu-rep --page raw --csv | python profiles/summarize_ncu_raw.py [title]
 
 One line per profiled launch: grid, duration, DRAM bytes (read + write), tensor-pipe / issue / DRAM / L2 / shared-memory utilisation,
-registers, occupancy, shared-memory bank conflicts.  Times under ncu are cold-cache and serialised (B200_PROFILING.md): use the shares."""
+registers, occupancy, shared-memory bank conflicts.  Times under ncu are cold-cache and serialised: use the shares."""
 import csv
 import sys
 

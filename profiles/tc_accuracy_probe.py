@@ -1,4 +1,4 @@
-"""Accuracy probe of the tcgen05 3xTF32 engine vs the fp32 SIMT engine against an fp64 reference (run on the GPU box)."""
+"""Accuracy probe of the wgmma 3xTF32 engine vs the fp32 SIMT engine against an fp64 reference (run on an H100)."""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from rl_x_b200.algorithms.ppo.b200.kernels import PpoKernels

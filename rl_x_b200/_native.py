@@ -165,7 +165,6 @@ _SIGNATURES = {
     "rlx_set_head_engine": (C.c_int, [C.c_int]),
     "rlx_set_gae_tma": (C.c_int, [C.c_int]),
     "rlx_set_autocast_bf16": (C.c_int, [C.c_int]),
-    "rlx_set_tc_pair": (C.c_int, [C.c_int, C.c_int]),
     "rlx_set_fused_tail": (C.c_int, [C.c_int]),
     "rlx_debug_ppo_head_gemm_f32": (C.c_int, [C.c_int64, C.c_int32, C.c_int32] + [C.c_void_p] * 11 + [C.c_float] * 3 + [C.c_int32] + [C.c_void_p] * 5),
     "rlx_get_gemm_engine": (C.c_int, []),

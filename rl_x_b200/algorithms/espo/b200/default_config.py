@@ -1,5 +1,5 @@
 """Same keys and defaults as rl_x/algorithms/espo/pytorch/default_config.py:4-30; `bf16_mixed_precision_training` defaults to
-    False (fp32 parity path), `compile_mode` is accepted and ignored, B200-specific keys appended."""
+    False (fp32 parity path), `compile_mode` is accepted and ignored, keys specific to this build appended."""
 from rl_x_b200.config_dict import config_from_defaults
 
 _DEFAULTS = (
@@ -24,7 +24,7 @@ _DEFAULTS = (
     ('nr_hidden_units', 256),
     ('evaluation_frequency', -1),
     ('evaluation_episodes', 10),
-    ('gemm_engine', "auto"),  # auto | simt (fp32 FFMA) | tcgen05 (3xTF32 tensor cores)
+    ('gemm_engine', "auto"),  # auto | simt (fp32 FFMA) | tcgen05 (historical name of the 3xTF32 wgmma tensor-core engine)
     ('rollout_noise', "philox"),  # philox (in-kernel counter-based normals) | torch (torch.randn on device, injected)
 )
 

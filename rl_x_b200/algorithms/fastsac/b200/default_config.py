@@ -34,7 +34,7 @@ _DEFAULTS = (
     ('logging_frequency', 40960),
     ('evaluation_frequency', -1),
     ('save_frequency', 4096000),  # -1 to disable
-    ('gemm_engine', "auto"),      # not a reference key: auto (the library's setting; exact-fp32 SIMT unless changed) | simt | tcgen05 (3xTF32)
+    ('gemm_engine', "auto"),      # not a reference key: auto (the library's setting; exact-fp32 SIMT unless changed) | simt | tcgen05 (historical name of the 3xTF32 wgmma tensor-core engine)
 )
 
 

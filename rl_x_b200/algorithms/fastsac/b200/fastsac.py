@@ -1,4 +1,4 @@
-"""FastSAC on B200 — mirrors rl_x/algorithms/fastsac/pytorch/fastsac.py (constructor, train(), test(), logging keys), fp32 path.
+"""FastSAC on the GPU — mirrors rl_x/algorithms/fastsac/pytorch/fastsac.py (constructor, train(), test(), logging keys), fp32 path.
 
 Host side: Python/PyTorch for device memory and the TORCH-interface environment; every compute step is a C-ABI call (include/rlx_b200.h):
 
@@ -8,7 +8,7 @@ Host side: Python/PyTorch for device memory and the TORCH-interface environment;
                  policy_loss_fn (fastsac.py:106-138)                                             rlx_fastsac_policy_update_f32
 
 Parameters are initialised exactly like the reference (the same torch modules built in the same order under torch.manual_seed(seed),
-fastsac.py:77-84) and live in the library's flat layout; action noise is torch.randn on the device.  Not built: bf16 autocast.  STATUS: on hardware since round 1 (tests/test_gpu_zzzz_fastsac.py); the same sources are checked in host emulation (tests/test_fastsac_emulation.py).
+fastsac.py:77-84) and live in the library's flat layout; action noise is torch.randn on the device.  Not built: bf16 autocast.  GPU tests: tests/test_gpu_zzzz_fastsac.py; the same sources are checked in host emulation (tests/test_fastsac_emulation.py).
 """
 import ctypes as C
 import logging
@@ -104,7 +104,7 @@ class FastSAC:
         rlx_logger.info(f"Using device: {self.device}")
 
         self.lib = nt.load()
-        engine = a.get("gemm_engine", "auto")   # dense layers: exact-fp32 SIMT, or the tcgen05 3xTF32 engine where it covers the product
+        engine = a.get("gemm_engine", "auto")   # dense layers: exact-fp32 SIMT, or the 3xTF32 wgmma engine ("tcgen05") where it covers the product
         if engine not in ("auto", "simt", "tcgen05"):
             raise ValueError("algorithm.gemm_engine must be auto, simt or tcgen05")
         if engine != "auto":

@@ -1,6 +1,6 @@
 """Same keys and defaults as rl_x/algorithms/ppo/pytorch/default_config.py:4-30.  Differences, all explicit:
     `bf16_mixed_precision_training` defaults to False (this build is the fp32 parity path), `compile_mode` is accepted and
-    ignored (no tracing compiler here), and three B200-specific keys are appended."""
+    ignored (no tracing compiler here), and three keys specific to this build are appended."""
 from rl_x_b200.config_dict import config_from_defaults
 
 _DEFAULTS = (
@@ -24,7 +24,7 @@ _DEFAULTS = (
     ('nr_hidden_units', 256),
     ('evaluation_frequency', -1),
     ('evaluation_episodes', 10),
-    ('gemm_engine', "auto"),  # auto | simt (fp32 FFMA) | tcgen05 (3xTF32 tensor cores)
+    ('gemm_engine', "auto"),  # auto | simt (fp32 FFMA) | tcgen05 (historical name of the 3xTF32 wgmma tensor-core engine)
     ('exact_global_permutation', True),  # multi-GPU: reference-exact global shuffle (ppo.py:273-276) vs per-rank local shuffles
     ('gradient_exchange', "peer"),  # multi-GPU: peer (library all-reduce kernel over NVLink peer memory) | nccl (torch.distributed)
     ('peer_exchange_algorithm', "auto"),  # auto = one_shot (measured fastest at 2 and 8 GPUs) | one_shot | two_shot (reduce-scatter / all-gather, experimental)

@@ -1,4 +1,4 @@
-"""PPO with the reference's plugin surface (rl_x/algorithms/ppo/pytorch/ppo.py), executed by hand-written sm_100a kernels.
+"""PPO with the reference's plugin surface (rl_x/algorithms/ppo/pytorch/ppo.py), executed by hand-written sm_90a kernels.
 
 Same constructor / train / test / save / load / general_properties contract and the same metric names as the reference
 class `PPO` (ppo.py:22-486).  What differs is where the work happens:

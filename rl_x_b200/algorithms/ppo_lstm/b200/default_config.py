@@ -25,7 +25,7 @@ _DEFAULTS = (
     ('nr_hidden_units', 256),
     ('evaluation_frequency', -1),
     ('evaluation_episodes', 10),
-    ('gemm_engine', "auto"),    # not a reference key: auto (the library's setting; exact-fp32 SIMT unless changed) | simt | tcgen05 (3xTF32)
+    ('gemm_engine', "auto"),    # not a reference key: auto (the library's setting; exact-fp32 SIMT unless changed) | simt | tcgen05 (historical name of the 3xTF32 wgmma tensor-core engine)
     ('use_cuda_graph', False),  # not a reference key: replay each minibatch update as one captured CUDA graph (same kernels, same order)
 )
 

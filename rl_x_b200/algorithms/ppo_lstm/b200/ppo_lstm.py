@@ -1,4 +1,4 @@
-"""PPO with an LSTM policy on B200 — mirrors rl_x/algorithms/ppo_lstm/flax/ppo_lstm.py (constructor, train(), test(), logging keys).
+"""PPO with an LSTM policy on the GPU — mirrors rl_x/algorithms/ppo_lstm/flax/ppo_lstm.py (constructor, train(), test(), logging keys).
 
 The reference is JAX/Flax; here the host side is Python/PyTorch (device memory, streams) and every compute step is a call into the
 C-ABI library (include/rlx_b200.h, "PPO + LSTM path"):
@@ -11,7 +11,7 @@ C-ABI library (include/rlx_b200.h, "PPO + LSTM path"):
 Differences that follow from the missing JAX runtime (all explicit): parameters are initialised with the same initialiser families
 from a torch generator (not jax.random), the action noise is torch.randn on the device, and the per-epoch env permutations come from
 the library's PCG64 stream — so runs are not seed-for-seed comparable with the reference; checkpoints are torch files with named
-tensors instead of Orbax trees.  STATUS: on hardware since round 1 (tests/test_gpu_zzz_ppo_lstm.py); the same sources are checked in host emulation (tests/test_lstm_emulation.py).
+tensors instead of Orbax trees.  GPU tests: tests/test_gpu_zzz_ppo_lstm.py; the same sources are checked in host emulation (tests/test_lstm_emulation.py).
 """
 import ctypes as C
 import logging
@@ -119,7 +119,7 @@ class PPO_LSTM:
         if len(self.os_shape) != 1 or len(self.as_shape) != 1:
             raise ValueError("rl_x_b200 PPO_LSTM supports flat observations and flat continuous actions only.")
         self.lib = nt.load()
-        engine = a.get("gemm_engine", "auto")   # dense layers: exact-fp32 SIMT, or the tcgen05 3xTF32 engine where it covers the product
+        engine = a.get("gemm_engine", "auto")   # dense layers: exact-fp32 SIMT, or the 3xTF32 wgmma engine ("tcgen05") where it covers the product
         if engine not in ("auto", "simt", "tcgen05"):
             raise ValueError("algorithm.gemm_engine must be auto, simt or tcgen05")
         if engine != "auto":

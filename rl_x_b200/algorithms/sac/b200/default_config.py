@@ -22,7 +22,7 @@ _DEFAULTS = (
     ('evaluation_frequency', -1),
     ('evaluation_episodes', 10),
     ('use_cuda_graph', True),  # replay the whole update (noise + ~58 kernels) as one CUDA graph
-    ('gemm_engine', "auto"),  # auto | simt (fp32 FFMA) | tcgen05 (3xTF32 tensor cores)
+    ('gemm_engine', "auto"),  # auto | simt (fp32 FFMA) | tcgen05 (historical name of the 3xTF32 wgmma tensor-core engine)
 )
 
 

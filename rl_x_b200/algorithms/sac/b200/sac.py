@@ -1,4 +1,4 @@
-"""SAC with the reference's plugin surface (rl_x/algorithms/sac/pytorch/sac.py), executed by the sm_100a library.
+"""SAC with the reference's plugin surface (rl_x/algorithms/sac/pytorch/sac.py), executed by the sm_90a library.
 
 Per environment step the reference does: act -> env.step -> replay add (host numpy) -> sample (2x rng.integers, 5 fancy-index gathers,
 5 H2D copies) -> critic_loss_fn -> Polyak loop over parameters -> policy_and_entropy_loss_fn -> 10 .item() syncs (sac.py:180-259).
@@ -493,7 +493,7 @@ class SAC:
         ov = model._optimizer_views()
         steps = [_load_adam_state(ck[f"{name}_optimizer_state_dict"], *ov[name], name) if f"{name}_optimizer_state_dict" in ck else 0
                  for name in ("policy", "q", "entropy")]
-        if "optimizer_flat" in ck:  # files written by round 1 of this build
+        if "optimizer_flat" in ck:  # files written by earlier versions of this build
             for k, v in ck["optimizer_flat"].items():
                 getattr(model, k).copy_(v)
         else:

@@ -1,8 +1,8 @@
-"""Builds the C-ABI CUDA library in-tree: rl_x_b200/lib/librlx_b200.so (sm_100a only).
+"""Builds the C-ABI CUDA library in-tree: rl_x_b200/lib/librlx_b200.so (sm_90a only).
 
     python -m rl_x_b200.build [--force] [--verbose]
 
-nvcc cross-compiles without a GPU.  The .so is git-ignored but travels with gpurun snapshots.
+nvcc cross-compiles without a GPU.  The .so and the objects are build products and stay out of git.
 """
 import hashlib
 import os
@@ -17,7 +17,7 @@ STAMP = os.path.join(LIB_DIR, "librlx_b200.stamp")
 INCLUDE = os.path.join(os.path.dirname(PKG_DIR), "include")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
 ]
@@ -89,7 +89,7 @@ def _compile_one(src, hdr_digest, verbose):
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA source for sm_100a (one nvcc process per translation unit, in parallel, unchanged units are reused) and link
+    """Compile every CUDA source for sm_90a (one nvcc process per translation unit, in parallel, unchanged units are reused) and link
     them into one shared library. Returns the path."""
     os.makedirs(OBJ_DIR, exist_ok=True)
     if not force and is_fresh():
@@ -120,7 +120,7 @@ def _build_locked(force, verbose):
     if errors:
         raise RuntimeError("\n".join(errors))
     tmp = LIB_PATH + ".tmp%d" % os.getpid()
-    cmd = [nvcc_path(), "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-Xcompiler", "-fPIC", "-o", tmp] + [o for o, _ in results]
+    cmd = [nvcc_path(), "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-Xcompiler", "-fPIC", "-o", tmp] + [o for o, _ in results]
     proc = subprocess.run(cmd, cwd=CSRC, capture_output=True, text=True)
     if proc.returncode != 0:
         if os.path.exists(tmp):

@@ -332,8 +332,7 @@ static int comm_allreduce(rlx_comm* c, float* out, int64_t n, void* stream, cons
     v.flags[r] = (unsigned long long*)c->peer[r];
     v.result[r] = (float*)(c->peer[r] + kFlagBytes + 2 * c->slot_bytes);
   }
-  // Two-shot only when asked for.  Measured inside the PPO epoch on 8 B200s (gpurun_out/r2_bench_8gpu*.json): 61 us per exchange against
-  // 49 us for the one-shot kernel - at 1.3 MB the second flag round costs more than the 8 MB of extra NVLink reads it saves.
+  // Two-shot only when asked for: at the ~1.3 MB of one PPO exchange the second flag round costs more than the extra peer reads it saves.
   const bool two_shot = c->algo == 2 && (c->world == 2 || c->world == 4 || c->world == 8);
   if (two_shot) {
     const int64_t n4c = std::max<int64_t>((n >> 2) / c->world, 1);

@@ -1,4 +1,4 @@
-// Shared helpers for the rlx_b200 C-ABI library (sm_100a).
+// Shared helpers for the rlx_b200 C-ABI library (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -143,14 +143,14 @@ extern "C" void rlx_emu_set_thread_order(int reverse) { rlx::g_emu_reverse = rev
 #include "common.cuh"
 #include "gemm_dispatch.cuh"
 namespace rlx {
-// dense layer of a dual-build source: exact-fp32 SIMT engine, or (rlx_set_aux_gemm_engine(1)) the tcgen05 3xTF32 engine where it covers the
+// dense layer of a dual-build source: exact-fp32 SIMT engine, or (rlx_set_aux_gemm_engine(1)) the wgmma 3xTF32 engine where it covers the
 // layout / epilogue / alignment.  a_rows / b_rows: rows of the operand tensors in memory (see run_gemm).  Single-CTA tensor kernels, and
 // only for products with at least half a tile in each output dimension: the skinny ones (heads, biases-as-GEMMs) carry no FLOPs worth
 // a TMA descriptor and stay on the SIMT engine.
 template <bool A_KMAJ, bool B_KMAJ, int EPI>
 static int aux_gemm(const GemmP& p, int batch, cudaStream_t st, int kclass, long long a_rows, long long b_rows) {
   if (g_aux_gemm_engine == 1 && p.M >= 64 && p.N >= 64 && p.K >= 32 && p.rowsum == nullptr) {
-    const int rc = tc_gemm(p, A_KMAJ, B_KMAJ, tc_epi_of<EPI>(), batch, kclass, a_rows, b_rows, 0, nullptr, 0, 0, st, 0);
+    const int rc = tc_gemm(p, A_KMAJ, B_KMAJ, tc_epi_of<EPI>(), batch, kclass, a_rows, b_rows, 0, nullptr, 0, 0, st);
     if (rc == RLX_OK) g_aux_tc_gemms.fetch_add(1, std::memory_order_relaxed);   // rlx_aux_tc_gemm_count(): evidence of which engine ran
     if (rc != RLX_ERR_UNSUPPORTED) return rc;
   }

@@ -1,4 +1,4 @@
-// One GEMM through the selected engine: tcgen05 3xTF32 when it covers the shape / alignment, exact-fp32 SIMT otherwise.
+// One GEMM through the selected engine: wgmma 3xTF32 when it covers the shape / alignment, exact-fp32 SIMT otherwise.
 #pragma once
 #include "gemm_simt.cuh"
 
@@ -6,13 +6,10 @@ namespace rlx {
 
 // gemm_tc.cu; returns RLX_ERR_UNSUPPORTED when a shape / alignment is not covered
 int tc_supported(const rlx_ppo_dims& d);
-// pair_bn: 0 = single-CTA kernels; 128 / 192 / 256 = CTA-pair kernel (cta_group::2, gemm_tc2.cu) with that tile width
 int tc_gemm(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int kclass, long long a_rows, long long b_rows, int n_main,
-            float* extra_col, long long extra_batch_off, long long extra_split_off, cudaStream_t stream, int pair_bn = 0);
+            float* extra_col, long long extra_batch_off, long long extra_split_off, cudaStream_t stream);
 int tc_gemm_t(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int kclass, long long a_rows, long long b_rows, int n_main,
-              float* extra_col, long long extra_batch_off, long long extra_split_off, cudaStream_t stream, int transpose_out, int m_main, int pair_bn = 0);
-int tc_pair_mode();     // 0 off, 1 weight-gradient GEMMs, 2 all large GEMMs
-int tc_pair_fwd_bn();   // pair tile width for forward / dX GEMMs (0 = single-CTA)
+              float* extra_col, long long extra_batch_off, long long extra_split_off, cudaStream_t stream, int transpose_out, int m_main);
 enum { TC_NONE = 0, TC_BIAS_TANH = 1, TC_DTANH = 2, TC_BIAS_RELU = 3, TC_DRELU = 4, TC_BIAS = 5 };
 
 template <int EPI>
@@ -23,9 +20,9 @@ constexpr int tc_epi_of() {
 
 // a_rows / b_rows: rows of the operand tensors as laid out in memory (TMA needs the true extents for its zero fill).
 template <bool A_KMAJ, bool B_KMAJ, int EPI>
-static int run_gemm(bool tc, const GemmP& g, int batch, cudaStream_t st, int kclass, long long a_rows, long long b_rows, int pair_bn = 0) {
+static int run_gemm(bool tc, const GemmP& g, int batch, cudaStream_t st, int kclass, long long a_rows, long long b_rows) {
   if (tc && g.rowsum == nullptr && g.K >= 32) {
-    const int rc = tc_gemm(g, A_KMAJ, B_KMAJ, tc_epi_of<EPI>(), batch, kclass, a_rows, b_rows, 0, nullptr, 0, 0, st, pair_bn);
+    const int rc = tc_gemm(g, A_KMAJ, B_KMAJ, tc_epi_of<EPI>(), batch, kclass, a_rows, b_rows, 0, nullptr, 0, 0, st);
     if (rc != RLX_ERR_UNSUPPORTED) return rc;
   }
   return launch_sgemm<A_KMAJ, B_KMAJ, EPI>(g, batch, st, kclass);

@@ -1,5 +1,5 @@
 // fp32 SIMT (FFMA) GEMM engine: 128x128x8 register-tiled kernel, double-buffered shared memory.
-// This is the exact-fp32 engine (bitwise fp32 FMA accumulation in k order); the tcgen05 3xTF32 engine in gemm_tc.cu
+// This is the exact-fp32 engine (bitwise fp32 FMA accumulation in k order); the wgmma 3xTF32 engine in gemm_tc.cu
 // is validated against it.  One template covers the three operand layouts the MLP needs:
 //   forward      C[m,n] = act(sum_k A[m,k] W[n,k] + b[n])           A k-major, B k-major   ("NT")
 //   backward dX  C[m,n] = (sum_k dZ[m,k] W[k,n]) * (1 - H[m,n]^2)    A k-major, B n-major   ("NN")

@@ -1,90 +1,107 @@
-// tcgen05 (5th-generation tensor core) GEMM engine with fp32-equivalent accuracy: 3xTF32 split.
+// Hopper tensor-core (wgmma) GEMM engine with fp32-equivalent accuracy: 3xTF32 split.
 //
-//   C[m,n] = epilogue( sum_k A(m,k) * B(n,k) ),  A, B, C fp32 in global memory, accumulation in fp32 in TMEM.
+//   C[m,n] = epilogue( sum_k A(m,k) * B(n,k) ),  A, B, C fp32 in global memory, accumulation in fp32 registers.
 //
-// Each fp32 operand x is used as  x = hi + lo  with hi = tf32(x) (the tensor core reads the top 19 bits of the fp32 word)
-// and lo = x - hi (exact in fp32); three MMAs per k-slice accumulate  hi*hi + hi*lo + lo*hi  (the lo*lo term is below fp32
+// Each fp32 operand x is used as  x = hi + lo  with hi = x with the low 13 mantissa bits cleared (an exact tf32 value) and
+// lo = x - hi (exact in fp32); three MMAs per k-slice accumulate  hi*hi + hi*lo + lo*hi  (the lo*lo term is below fp32
 // resolution).  That is the accuracy class of an fp32 FMA loop (SURVEY.md §7a: single-pass TF32 misses the 1e-5 loss-parity bar,
 // 3xTF32 does not) at one third of the TF32 tensor rate.
 //
-// Structure (one persistent CTA per SM, 448 threads, static tile schedule):
-//   warp 0      TMA producer: cp.async.bulk.tensor 2-D tiles (SWIZZLE_128B) of raw fp32 A and B into a shared-memory ring
-//   warps 2-5   splitter: read the raw tiles, write the lo tiles (same swizzled layout) next to them, fence.proxy.async
-//   warp 1      MMA issuer: ONE thread issues tcgen05.mma.cta_group::1.kind::tf32 (3 per k-slice of 8), tcgen05.commit frees the
-//               ring slot / publishes the accumulator
-//   warps 6-13  epilogue (two warp-groups): tcgen05.ld the 128 x BN fp32 accumulator out of TMEM (double-buffered: the next tile's MMAs overlap),
-//               bias+tanh / tanh' / plain, 128-bit global stores
-// Operand layouts: K-major (row = m or n, 32 consecutive k = one 128-byte swizzle row) or MN-major (row = k, 32 consecutive
-// m/n per 128-byte row; used by the weight-gradient GEMMs whose reduction runs over the minibatch rows).  Out-of-bounds parts
-// of a box are zero-filled by TMA, so M / N / K tails need no special code in the main loop.
+// Structure (one persistent CTA per SM, 384 threads = 3 warpgroups, static tile schedule, 128 x 128 output tiles):
+//   warpgroup 0   thread 0 issues cp.async.bulk.tensor 2-D tiles (SWIZZLE_128B) of raw fp32 A and B into a 3-stage ring, running ahead
+//                 of the conversion; all 128 threads then write the hi and lo tiles of both operands, K-major and 128-byte swizzled
+//                 (the only layout wgmma accepts for tf32), into a 2-stage operand ring and fence.proxy.async it for the tensor core
+//   warpgroups 1, 2   rows 0-63 / 64-127 of the tile: wgmma.mma_async m64n128k8 tf32 (3 per k-slice of 8), then the epilogue straight
+//                 from the accumulator registers: bias+tanh / tanh' / relu / plain, stores to C (or C^T)
+// Operand layouts in global memory: K-major (row = m or n, 32 consecutive k = one 128-byte swizzle row) or MN-major (row = k, 32
+// consecutive m/n per 128-byte row; used by the weight-gradient GEMMs whose reduction runs over the minibatch rows).  The converter
+// transposes MN-major tiles to K-major.  Out-of-bounds parts of a box are zero-filled by TMA, so M / N / K tails need no special code
+// in the main loop.
+#include "gemm_dispatch.cuh"
 #include "gemm_tc_common.cuh"
 
 namespace rlx {
 namespace tc {
 
-// TMEM: every output tile owns TWO fp32 accumulators of BN columns: `main` collects hi*hi, `corr` collects hi*lo + lo*hi.
-// The tensor core adds into an accumulator with round-toward-zero (measured: error grows by ~0.3 ulp per MMA, profiles/
-// tc_accuracy_probe.py), so the tiny correction terms must not touch the main accumulator; the epilogue adds the two in fp32 RN.
-// BN = 256 -> one tile in flight (512 columns); BN = 128 -> double-buffered (2 x 256 columns: next tile's MMAs overlap the epilogue).
-template <int BN>
+// The main product and the correction terms go to separate accumulators: tiny correction terms added into the large running sum
+// would lose their low bits to the tensor core's accumulation rounding; the epilogue adds the two in fp32 round-to-nearest.
 struct Cfg {
   static constexpr int A_BYTES = BM * BK * 4;                   // 16 KB
-  static constexpr int B_BYTES = BN * BK * 4;                   // 16 / 32 KB
-  static constexpr int STAGE_BYTES = 2 * (A_BYTES + B_BYTES);   // raw + lo
-  static constexpr int STAGES = (BN == 256) ? 2 : 3;
-  static constexpr int ACC_STAGES = (BN == 256) ? 1 : 2;
-  static constexpr int TMEM_COLS = ACC_STAGES * 2 * BN;         // 512
-  static constexpr int AUX_BYTES = 1024 /*barriers etc.*/ + EPI_WARPS * 32 * 33 * 4 /*epilogue transpose staging, one [32][33] tile per warp*/;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + AUX_BYTES + 1024 /*alignment slack*/;
+  static constexpr int B_BYTES = BN * BK * 4;                   // 16 KB
+  static constexpr int RAW_BYTES = A_BYTES + B_BYTES;           // raw stage: [A | B] as TMA wrote them
+  static constexpr int OP_BYTES = 2 * RAW_BYTES;                // operand stage: [hi A | hi B | lo A | lo B], K-major swizzled
+  static constexpr int RAW_STAGES = 3, OP_STAGES = 2;
+  static constexpr int SMEM_BYTES = RAW_STAGES * RAW_BYTES + OP_STAGES * OP_BYTES + 1024 /*barriers*/ + 1024 /*alignment slack*/;
 };
+static_assert(Cfg::SMEM_BYTES <= 227 * 1024, "shared memory of one H100 block");
+
+// One operand tile (ROWS x BK) from its raw stage to K-major swizzled hi / lo tiles.  In the 128-byte swizzle every 16-byte chunk
+// (4 k-values) c of row r sits at r * 128 + ((c ^ (r & 7)) << 4).  Thread t of the warpgroup handles chunks t, t + 128, ...
+template <bool KMAJ, bool BF16, int ROWS>
+__device__ __forceinline__ void convert_tile(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int t) {
+  constexpr uint32_t HI = 0xFFFFE000u;
+  if (KMAJ) {
+    // TMA wrote the tile in exactly the target layout: an element-wise pass
+#pragma unroll 4
+    for (int i = t; i < ROWS * 8; i += 128) {
+      const uint4 v = reinterpret_cast<const uint4*>(raw)[i];
+      const uint4 h = make_uint4(v.x & HI, v.y & HI, v.z & HI, v.w & HI);
+      reinterpret_cast<uint4*>(hi)[i] = h;
+      if (!BF16)
+        reinterpret_cast<float4*>(lo)[i] = make_float4(__uint_as_float(v.x) - __uint_as_float(h.x), __uint_as_float(v.y) - __uint_as_float(h.y),
+                                                       __uint_as_float(v.z) - __uint_as_float(h.z), __uint_as_float(v.w) - __uint_as_float(h.w));
+    }
+  } else {
+    // ROWS / 32 boxes of [BK k-rows][32 mn] (4 KB each, swizzled the same way with k as the row).  A warp handles 32 consecutive mn of
+    // one k-chunk: its reads of one k-row hit 32 different banks, its 16-byte writes are conflict-free per quarter warp.
+#pragma unroll 2
+    for (int i = t; i < ROWS * 8; i += 128) {
+      const int mn = i % ROWS, kc = i / ROWS;
+      const uint8_t* box = raw + (mn >> 5) * (BK * 128);
+      const int c = (mn & 31) >> 2, e = mn & 3;
+      uint32_t v[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int k = kc * 4 + q;
+        v[q] = *reinterpret_cast<const uint32_t*>(box + k * 128 + ((c ^ (k & 7)) << 4) + e * 4);
+      }
+      const int off = mn * 128 + ((kc ^ (mn & 7)) << 4);
+      const uint4 h = make_uint4(v[0] & HI, v[1] & HI, v[2] & HI, v[3] & HI);
+      *reinterpret_cast<uint4*>(hi + off) = h;
+      if (!BF16)
+        *reinterpret_cast<float4*>(lo + off) = make_float4(__uint_as_float(v[0]) - __uint_as_float(h.x), __uint_as_float(v[1]) - __uint_as_float(h.y),
+                                                           __uint_as_float(v[2]) - __uint_as_float(h.z), __uint_as_float(v[3]) - __uint_as_float(h.w));
+    }
+  }
+}
 
 // BF16: the bf16-autocast variant (single-pass MMAs on bf16-valued operands, bf16 roundings in the epilogue), a compile-time switch so that
 // the fp32-equivalent kernels carry none of it
-template <int BN, bool A_KMAJ, bool B_KMAJ, int EPI, bool BF16>
+template <bool A_KMAJ, bool B_KMAJ, int EPI, bool BF16>
 __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
                                                                  const __grid_constant__ CUtensorMap tmap_b, const TcParams p) {
-  using C_ = Cfg<BN>;
-  constexpr int STAGES = C_::STAGES;
-  constexpr int ACC_STAGES = C_::ACC_STAGES;
+  constexpr int RAW_STAGES = Cfg::RAW_STAGES, OP_STAGES = Cfg::OP_STAGES;
   extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment as an OFFSET on the __shared__ pointer: a round trip through uintptr_t makes the compiler lose the shared
-  // address space and emit generic LD/ST for every access below (seen in profiles/r01_tc_minibatch_ncu_v2: splitter stalled on LD.E.128)
+  // 1024-byte alignment (swizzle atoms) as an OFFSET on the __shared__ pointer: a round trip through uintptr_t makes the compiler lose
+  // the shared address space and emit generic loads / stores
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* aux = smem + STAGES * C_::STAGE_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);            // [STAGES]  TMA landed
-  uint64_t* split_bar = full_bar + STAGES;                          // [STAGES]  lo tiles written
-  uint64_t* empty_bar = split_bar + STAGES;                         // [STAGES]  MMAs of the slot retired
-  uint64_t* tmem_full_bar = empty_bar + STAGES;                     // [ACC_STAGES]
-  uint64_t* tmem_empty_bar = tmem_full_bar + ACC_STAGES;            // [ACC_STAGES]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + ACC_STAGES);
-  float* stage_smem = reinterpret_cast<float*>(aux + 1024);
+  uint8_t* ops = smem + RAW_STAGES * Cfg::RAW_BYTES;
+  uint64_t* raw_full = reinterpret_cast<uint64_t*>(ops + OP_STAGES * Cfg::OP_BYTES);  // [RAW_STAGES]  TMA landed
+  uint64_t* op_full = raw_full + RAW_STAGES;                                          // [OP_STAGES]   hi / lo tiles written
+  uint64_t* op_empty = op_full + OP_STAGES;                                           // [OP_STAGES]   wgmmas of the slot retired
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_b);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < STAGES; ++s) {
-        mbar_init(&full_bar[s], 1);
-        mbar_init(&split_bar[s], 4);
-        mbar_init(&empty_bar[s], 1);
-      }
-      for (int a = 0; a < ACC_STAGES; ++a) {
-        mbar_init(&tmem_full_bar[a], 1);
-        mbar_init(&tmem_empty_bar[a], EPI_WARPS);
-      }
-      fence_barrier_init();
+    for (int s = 0; s < RAW_STAGES; ++s) mbar_init(&raw_full[s], 1);
+    for (int s = 0; s < OP_STAGES; ++s) {
+      mbar_init(&op_full[s], 1);
+      mbar_init(&op_empty[s], 8);  // one arrival per consumer warp
     }
-    __syncwarp();
-    tmem_alloc(tmem_ptr_smem, C_::TMEM_COLS);
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   const int tiles_per_z = p.tiles_m * p.tiles_n;
   const int num_tiles = tiles_per_z * p.batch * p.splits;
@@ -100,254 +117,163 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
     nkb = (kend - kbeg + BK - 1) / BK;
   };
 
-  if (warp == 0) {
-    // ===================================================== TMA producer
-    if (lane == 0) {
-      int s = 0;
-      uint32_t ph = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+  if (warp < 4) {
+    // ===================================================== TMA (thread 0) + hi / lo converter (warpgroup 0)
+    const int t = threadIdx.x;
+    // load cursor: the k-blocks of this CTA's tiles in consumption order; a raw slot is refilled as soon as the converter is done with it
+    int ld_tile = blockIdx.x, ld_kb = 0, ld_count = 0;
+    auto load_next = [&]() {
+      while (ld_tile < num_tiles) {
         int zb, zs, m0, n0, kbeg, nkb;
-        tile_coords(tile, zb, zs, m0, n0, kbeg, nkb);
-        auto issue = [&](int kb, bool prefetch_only, uint8_t* sa, uint8_t* sb, uint64_t* bar) {
-          const int k0 = kbeg + kb * BK;
-          if (A_KMAJ) {
-            const int c0 = p.a_k_off * zb + k0, c1 = p.a_mn_off * zb + m0;
-            if (prefetch_only) tma_prefetch_2d(&tmap_a, c0, c1); else tma_load_2d(&tmap_a, bar, sa, c0, c1);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BM / 32; ++j) {
-              const int c0 = p.a_mn_off * zb + m0 + 32 * j, c1 = p.a_k_off * zb + k0;
-              if (prefetch_only) tma_prefetch_2d(&tmap_a, c0, c1); else tma_load_2d(&tmap_a, bar, sa + j * (BK * 128), c0, c1);
-            }
-          }
-          if (B_KMAJ) {
-            const int c0 = p.b_k_off * zb + k0, c1 = p.b_mn_off * zb + n0;
-            if (prefetch_only) tma_prefetch_2d(&tmap_b, c0, c1); else tma_load_2d(&tmap_b, bar, sb, c0, c1);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BN / 32; ++j) {
-              const int c0 = p.b_mn_off * zb + n0 + 32 * j, c1 = p.b_k_off * zb + k0;
-              if (prefetch_only) tma_prefetch_2d(&tmap_b, c0, c1); else tma_load_2d(&tmap_b, bar, sb + j * (BK * 128), c0, c1);
-            }
-          }
-        };
-        constexpr int PF = STAGES + 3;  // L2 prefetch distance in k-blocks
-        for (int kb = 0; kb < min(PF, nkb); ++kb) issue(kb, true, nullptr, nullptr, nullptr);
-        for (int kb = 0; kb < nkb; ++kb) {
-          if (kb + PF < nkb) issue(kb + PF, true, nullptr, nullptr, nullptr);
-          mbar_wait(&empty_bar[s], ph ^ 1);
-          uint8_t* st = smem + s * C_::STAGE_BYTES;
-          mbar_arrive_expect_tx(&full_bar[s], C_::A_BYTES + C_::B_BYTES);
-          issue(kb, false, st, st + C_::A_BYTES, &full_bar[s]);
-          if (++s == STAGES) { s = 0; ph ^= 1; }
+        tile_coords(ld_tile, zb, zs, m0, n0, kbeg, nkb);
+        if (ld_kb >= nkb) {
+          ld_tile += gridDim.x;
+          ld_kb = 0;
+          continue;
         }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer (single thread)
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(BN, !A_KMAJ, !B_KMAJ);
-      // K-major: LBO unused (1), SBO = 8 rows * 128 B.  MN-major: LBO = stride between 32-wide MN atoms, SBO = 8 k-rows * 128 B.
-      constexpr uint32_t A_LBO = A_KMAJ ? 16u : (uint32_t)(BK * 128), B_LBO = B_KMAJ ? 16u : (uint32_t)(BK * 128);
-      constexpr uint32_t A_SBO = A_KMAJ ? 1024u : 512u, B_SBO = B_KMAJ ? 1024u : 512u;
-      constexpr uint32_t A_LT = A_KMAJ ? 2u : 1u, B_LT = B_KMAJ ? 2u : 1u;
-      constexpr uint32_t A_KSTEP = A_KMAJ ? (UMMA_K * 4) : (UMMA_K * 128), B_KSTEP = B_KMAJ ? (UMMA_K * 4) : (UMMA_K * 128);
-      // stage-0 descriptors of the raw A / B tiles; the lo tiles sit A_BYTES + B_BYTES further in the same stage
-      const uint32_t s0 = smem_u32(smem);
-      const uint64_t da0 = make_smem_desc(s0, A_LBO, A_SBO, A_LT);
-      const uint64_t db0 = make_smem_desc(s0 + C_::A_BYTES, B_LBO, B_SBO, B_LT);
-      constexpr uint64_t LO_OFF = (uint64_t)((C_::A_BYTES + C_::B_BYTES) >> 4);
-      int s = 0, acc = 0;
-      uint32_t ph = 0, acc_ph = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        int zb, zs, m0, n0, kbeg, nkb;
-        tile_coords(tile, zb, zs, m0, n0, kbeg, nkb);
-        mbar_wait(&tmem_empty_bar[acc], acc_ph ^ 1);
-        tc_fence_after();
-        const uint32_t d_main = tmem_base + (uint32_t)(acc * 2 * BN);
-        const uint32_t d_corr = d_main + (uint32_t)BN;
-        for (int kb = 0; kb < nkb; ++kb) {
-          mbar_wait(&split_bar[s], ph);  // the splitter passed full_bar[s] before arriving here: TMA data + lo tiles are both in place
-          tc_fence_after();
-          // descriptors differ from the stage-0 / slice-0 ones only in the 14-bit start-address field (units of 16 bytes): one add each
-          const uint64_t soff = (uint64_t)((uint32_t)(s * C_::STAGE_BYTES) >> 4);
+        const int slot = ld_count % RAW_STAGES;
+        uint8_t* sa = smem + slot * Cfg::RAW_BYTES;
+        uint8_t* sb = sa + Cfg::A_BYTES;
+        uint64_t* bar = &raw_full[slot];
+        const int k0 = kbeg + ld_kb * BK;
+        mbar_arrive_expect_tx(bar, Cfg::RAW_BYTES);
+        if (A_KMAJ) {
+          tma_load_2d(&tmap_a, bar, sa, p.a_k_off * zb + k0, p.a_mn_off * zb + m0);
+        } else {
 #pragma unroll
-          for (int kk = 0; kk < BK / UMMA_K; ++kk) {
-            const uint64_t da = da0 + soff + (uint64_t)((kk * A_KSTEP) >> 4);
-            const uint64_t db = db0 + soff + (uint64_t)((kk * B_KSTEP) >> 4);
-            const uint64_t da_lo = da + LO_OFF;
-            const uint64_t db_lo = db + LO_OFF;
-            const uint32_t accum = (kb | kk) != 0 ? 1u : 0u;
-            if (!BF16) {
-              umma_tf32(d_corr, da_lo, db, idesc, accum);  // lo * hi   } small terms, own accumulator
-              umma_tf32(d_corr, da, db_lo, idesc, 1u);     // hi * lo   }
-            }
-            umma_tf32(d_main, da, db, idesc, accum);       // hi * hi  (bf16-valued operands: the whole product)
-          }
-          umma_commit(&empty_bar[s]);  // slot reusable once these MMAs have read it
-          if (++s == STAGES) { s = 0; ph ^= 1; }
+          for (int j = 0; j < BM / 32; ++j) tma_load_2d(&tmap_a, bar, sa + j * (BK * 128), p.a_mn_off * zb + m0 + 32 * j, p.a_k_off * zb + k0);
         }
-        umma_commit(&tmem_full_bar[acc]);  // accumulators complete
-        if (++acc == ACC_STAGES) { acc = 0; acc_ph ^= 1; }
+        if (B_KMAJ) {
+          tma_load_2d(&tmap_b, bar, sb, p.b_k_off * zb + k0, p.b_mn_off * zb + n0);
+        } else {
+#pragma unroll
+          for (int j = 0; j < BN / 32; ++j) tma_load_2d(&tmap_b, bar, sb + j * (BK * 128), p.b_mn_off * zb + n0 + 32 * j, p.b_k_off * zb + k0);
+        }
+        ++ld_kb;
+        ++ld_count;
+        return;
       }
-    }
-  } else if (warp >= SPLIT_WARP0 && warp < EPI_WARP0) {
-    // ===================================================== splitter: lo = x - tf32_trunc(x)
-    const int t = threadIdx.x - SPLIT_WARP0 * 32;  // 0..127
-    constexpr int NV = (C_::A_BYTES + C_::B_BYTES) / 16;  // float4 chunks per stage (raw A and raw B are contiguous)
-    int s = 0;
-    uint32_t ph = 0;
+    };
+    if (t == 0)
+      for (int i = 0; i < RAW_STAGES; ++i) load_next();
+    int rs = 0, os = 0;
+    uint32_t rph = 0, oph = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int zb, zs, m0, n0, kbeg, nkb;
       tile_coords(tile, zb, zs, m0, n0, kbeg, nkb);
       for (int kb = 0; kb < nkb; ++kb) {
-        mbar_wait(&full_bar[s], ph);
-        const uint4* raw = reinterpret_cast<const uint4*>(smem + s * C_::STAGE_BYTES);
-        float4* lo = reinterpret_cast<float4*>(smem + s * C_::STAGE_BYTES + C_::A_BYTES + C_::B_BYTES);
-#pragma unroll 8
-        for (int i = t; i < (BF16 ? 0 : NV); i += 128) {
-          const uint4 v = raw[i];
-          float4 o;
-          o.x = __uint_as_float(v.x) - __uint_as_float(v.x & 0xFFFFE000u);
-          o.y = __uint_as_float(v.y) - __uint_as_float(v.y & 0xFFFFE000u);
-          o.z = __uint_as_float(v.z) - __uint_as_float(v.z & 0xFFFFE000u);
-          o.w = __uint_as_float(v.w) - __uint_as_float(v.w & 0xFFFFE000u);
-          lo[i] = o;
-        }
+        mbar_wait(&raw_full[rs], rph);
+        mbar_wait(&op_empty[os], oph ^ 1);
+        const uint8_t* raw = smem + rs * Cfg::RAW_BYTES;
+        uint8_t* op = ops + os * Cfg::OP_BYTES;
+        convert_tile<A_KMAJ, BF16, BM>(raw, op, op + Cfg::RAW_BYTES, t);
+        convert_tile<B_KMAJ, BF16, BN>(raw + Cfg::A_BYTES, op + Cfg::A_BYTES, op + Cfg::RAW_BYTES + Cfg::A_BYTES, t);
         fence_proxy_async();  // generic-proxy writes -> visible to the tensor core's async-proxy reads
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&split_bar[s]);
-        if (++s == STAGES) { s = 0; ph ^= 1; }
+        named_bar_sync(1, 128);  // the whole warpgroup is done with raw slot rs and has written operand slot os
+        if (t == 0) {
+          mbar_arrive(&op_full[os]);
+          load_next();  // refills raw slot rs
+        }
+        if (++rs == RAW_STAGES) { rs = 0; rph ^= 1; }
+        if (++os == OP_STAGES) { os = 0; oph ^= 1; }
       }
     }
   } else {
-    // ===================================================== epilogue: TMEM -> registers -> smem transpose -> coalesced global
-    // tcgen05.ld hands each thread 32 consecutive columns of ONE accumulator row.  Writing that straight out would touch 32
-    // different 128-byte lines per instruction, so the 32x32 chunk is transposed through a padded shared-memory tile: afterwards
-    // lane = column, and every global load (aux) / store (C) of a warp is one fully coalesced 128-byte row segment.
-    const int q = warp & 3;               // TMEM lane quarter this warp may access
-    float* tile = stage_smem + (warp - EPI_WARP0) * (32 * 33);
-    int acc = 0;
-    uint32_t acc_ph = 0;
-    for (int tile_i = blockIdx.x; tile_i < num_tiles; tile_i += gridDim.x) {
+    // ===================================================== wgmma consumers + epilogue (warpgroups 1, 2)
+    const int cw = (warp >> 2) - 1;  // rows 64 * cw .. 64 * cw + 63 of the tile
+    float acc[64], cor[64];
+    int os = 0;
+    uint32_t oph = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int zb, zs, m0, n0, kbeg, nkb;
-      tile_coords(tile_i, zb, zs, m0, n0, kbeg, nkb);
-      mbar_wait(&tmem_full_bar[acc], acc_ph);
-      tc_fence_after();
-      const int row0 = m0 + q * 32;
+      tile_coords(tile, zb, zs, m0, n0, kbeg, nkb);
+      for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait(&op_full[os], oph);
+        const uint32_t op = smem_u32(ops + os * Cfg::OP_BYTES);
+        const uint64_t da = make_smem_desc(op + cw * 64 * 128), db = make_smem_desc(op + Cfg::A_BYTES);
+        const uint64_t da_lo = make_smem_desc(op + Cfg::RAW_BYTES + cw * 64 * 128), db_lo = make_smem_desc(op + Cfg::RAW_BYTES + Cfg::A_BYTES);
+        fence_acc(acc);
+        if (!BF16) fence_acc(cor);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < BK / WG_K; ++kk) {
+          // advancing along k inside the 128-byte swizzle row: the descriptors differ only in the start address (units of 16 bytes)
+          const uint64_t ko = (uint64_t)((kk * WG_K * 4) >> 4);
+          const uint32_t accum = (kb | kk) != 0 ? 1u : 0u;
+          if (!BF16) {
+            wgmma_tf32_m64n128k8(cor, da_lo + ko, db + ko, accum);  // lo * hi   } small terms, own accumulator
+            wgmma_tf32_m64n128k8(cor, da + ko, db_lo + ko, 1u);     // hi * lo   }
+          }
+          wgmma_tf32_m64n128k8(acc, da + ko, db + ko, accum);       // hi * hi  (bf16-valued operands: the whole product)
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        fence_acc(acc);
+        if (!BF16) fence_acc(cor);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&op_empty[os]);
+        if (++os == OP_STAGES) { os = 0; oph ^= 1; }
+      }
+
+      // ---- epilogue.  Accumulator layout of wgmma m64nN f32: register j of lane l in warp w (of the warpgroup) holds row
+      // 16 w + l / 4 + 8 ((j >> 1) & 1), column 8 (j >> 2) + 2 (l & 3) + (j & 1).
+      const int r_base = m0 + cw * 64 + (warp & 3) * 16 + (lane >> 2);
+      const int c_base = n0 + 2 * (lane & 3);
       float* cbase = p.C + p.c_batch_off * zb + p.c_split_off * zs;
+      float* ebase = p.extra_col != nullptr ? p.extra_col + p.extra_batch_off * zb + p.extra_split_off * zs : nullptr;
       constexpr bool HAS_AUX = (EPI == TC_EPI_DTANH || EPI == TC_EPI_DRELU);
       constexpr bool HAS_BIAS = (EPI == TC_EPI_BIAS_TANH || EPI == TC_EPI_BIAS_RELU || EPI == TC_EPI_BIAS);
       const float* abase = HAS_AUX ? (p.aux + p.aux_batch_off * zb) : nullptr;
       const float* bias = HAS_BIAS ? (p.bias + p.bias_batch_off * zb) : nullptr;
-      const int rows_valid = min(32, p.M - row0);  // warp-uniform
-      const int eg = (warp - EPI_WARP0) >> 2;  // epilogue warp-group
-#pragma unroll 1
-      for (int c = eg; c < BN / 32; c += EPI_WARPS / 4) {
-        uint32_t r[32], rc[32];
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * 2 * BN + c * 32);
-        tmem_ld_32x32b_x32(taddr, r);
-        tmem_ld_32x32b_x32(taddr + BN, rc);
-        tmem_ld_wait();
-        const int nb = n0 + c * 32;
-        if (p.transpose_out) {
-          // transposed store: each lane owns one accumulator row m, so for a fixed column n the warp writes 32 consecutive
-          // floats of C^T (coalesced) straight from the TMEM registers - no shared-memory transpose needed
-          const int m = row0 + lane;
-          if (m < p.M) {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const int n = nb + j;
-              const float v = BF16 ? __uint_as_float(r[j]) : __uint_as_float(r[j]) + __uint_as_float(rc[j]);
-              if (n < p.N) {
-                if (m < p.m_main) cbase[(long long)n * p.ldc + m] = v;
-                else if (m == p.m_main && p.extra_col != nullptr) p.extra_col[p.extra_batch_off * zb + p.extra_split_off * zs + n] = v;
-              }
-            }
-          }
+      for (int j = 0; j < 64; ++j) {
+        const int m = r_base + 8 * ((j >> 1) & 1);
+        const int n = c_base + 8 * (j >> 2) + (j & 1);
+        if (m >= p.M || n >= p.N) continue;
+        float x = BF16 ? acc[j] : acc[j] + cor[j];  // main + correction (fp32 RN)
+        if (p.transpose_out) {
+          if (m < p.m_main) cbase[(long long)n * p.ldc + m] = x;
+          else if (m == p.m_main && ebase != nullptr) ebase[n] = x;
           continue;
         }
-        if (rows_valid > 0 && nb < p.N) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)  // main + correction (fp32 RN); single-pass mode never wrote the correction accumulator
-            tile[lane * 33 + j] = BF16 ? __uint_as_float(r[j]) : __uint_as_float(r[j]) + __uint_as_float(rc[j]);
-          __syncwarp();
-          const int n = nb + lane;
-          const bool n_ok = n < p.N;
-          float bv = 0.f;
-          if (HAS_BIAS && n_ok) bv = bias[n];
-          // Math is unconditional and fully unrolled (32 independent chains per lane: a branch per row would serialise the
-          // ~40-instruction tanhf sequences); only the global accesses are predicated.  Rows >= rows_valid hold zeros.
-          float x[32];
-#pragma unroll
-          for (int rr = 0; rr < 32; ++rr) x[rr] = tile[rr * 33 + lane];
-          if (HAS_AUX) {
-            float hv[32];
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr) hv[rr] = (rr < rows_valid && n_ok) ? abase[(long long)(row0 + rr) * p.ldaux + n] : 0.f;
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr)  // bf16 mode: linear-backward output rounded to bf16, then tanh_backward rounded to bf16
-              x[rr] = (EPI == TC_EPI_DTANH) ? bf16r_if(bf16r_if(x[rr], BF16) * (1.f - hv[rr] * hv[rr]), BF16) : ((hv[rr] > 0.f) ? x[rr] : 0.f);
-          }
-          if (HAS_BIAS) {
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr) {
-              const float z = (EPI == TC_EPI_BIAS_RELU) ? x[rr] + bv : bf16r_if(x[rr] + bv, BF16);  // bf16 mode: Linear output is a bf16 tensor
-              x[rr] = (EPI == TC_EPI_BIAS_TANH) ? bf16r_if(tanh_fast(z), BF16) : ((EPI == TC_EPI_BIAS_RELU) ? fmaxf(z, 0.f) : z);
-            }
-          }
-          if (n < p.n_main) {
-            float* cp = cbase + (long long)row0 * p.ldc + n;
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr)
-              if (rr < rows_valid) cp[(long long)rr * p.ldc] = x[rr];
-          } else if (n == p.n_main && n_ok && p.extra_col != nullptr) {
-            float* ep = p.extra_col + p.extra_batch_off * zb + p.extra_split_off * zs + row0;
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr)
-              if (rr < rows_valid) ep[rr] = x[rr];
-          }
-          __syncwarp();
+        if (HAS_AUX) {
+          const float h = abase[(long long)m * p.ldaux + n];
+          // bf16 mode: linear-backward output rounded to bf16, then tanh_backward rounded to bf16
+          x = (EPI == TC_EPI_DTANH) ? bf16r_if(bf16r_if(x, BF16) * (1.f - h * h), BF16) : ((h > 0.f) ? x : 0.f);
         }
+        if (HAS_BIAS) {
+          const float z = (EPI == TC_EPI_BIAS_RELU) ? x + bias[n] : bf16r_if(x + bias[n], BF16);  // bf16 mode: Linear output is a bf16 tensor
+          x = (EPI == TC_EPI_BIAS_TANH) ? bf16r_if(tanh_fast(z), BF16) : ((EPI == TC_EPI_BIAS_RELU) ? fmaxf(z, 0.f) : z);
+        }
+        if (n < p.n_main) cbase[(long long)m * p.ldc + n] = x;
+        else if (n == p.n_main && ebase != nullptr) ebase[m] = x;
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty_bar[acc]);
-      if (++acc == ACC_STAGES) { acc = 0; acc_ph ^= 1; }
     }
-  }
-
-  // ---- teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, C_::TMEM_COLS);
   }
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-template <int BN, bool A_KMAJ, bool B_KMAJ, int EPI, bool BF16 = false>
+template <bool A_KMAJ, bool B_KMAJ, int EPI, bool BF16 = false>
 static int launch_cfg(const TcOperand& A, const TcOperand& B, TcParams p, int kclass, cudaStream_t stream) {
   CUtensorMap ta, tb;
-  int rc = make_tmap(&ta, A.base, A.rows, A.cols, A.ld, 32, A_KMAJ ? BM : BK, A_KMAJ);
+  int rc = make_tmap(&ta, A.base, A.rows, A.cols, A.ld, 32, A_KMAJ ? BM : BK);
   if (rc) return rc;
-  rc = make_tmap(&tb, B.base, B.rows, B.cols, B.ld, 32, B_KMAJ ? BN : BK, B_KMAJ);
+  rc = make_tmap(&tb, B.base, B.rows, B.cols, B.ld, 32, B_KMAJ ? BN : BK);
   if (rc) return rc;
   p.tiles_m = (int)ceil_div(p.M, BM);
   p.tiles_n = (int)ceil_div(p.N, BN);
   const long long tiles = (long long)p.tiles_m * p.tiles_n * p.batch * p.splits;
   if (tiles <= 0) return RLX_OK;
-  auto kern = tc_gemm_kernel<BN, A_KMAJ, B_KMAJ, EPI, BF16>;
+  auto kern = tc_gemm_kernel<A_KMAJ, B_KMAJ, EPI, BF16>;
   static bool attr_done = false;
   if (!attr_done) {
-    RLX_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM_BYTES));
+    RLX_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     attr_done = true;
   }
   const unsigned grid = (unsigned)std::min<long long>(tiles, sm_count());
   const double flops = 2.0 * p.M * p.N * (double)p.K * p.batch;
   const double bytes = 4.0 * p.batch * ((double)p.M * p.K + (double)p.N * p.K + (double)p.M * p.N * p.splits);
-  RLX_LAUNCH_C(kclass, flops, bytes, kern, grid, NUM_THREADS, Cfg<BN>::SMEM_BYTES, stream, ta, tb, p);
+  RLX_LAUNCH_C(kclass, flops, bytes, kern, grid, NUM_THREADS, Cfg::SMEM_BYTES, stream, ta, tb, p);
   return RLX_OK;
 }
 
@@ -364,26 +290,13 @@ static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 
 // Generic front end over the SIMT engine's GemmP (same meaning of every field).  Supported: all strides multiples of 4 floats,
 // 16-byte aligned bases, batch strides that are pure row or column offsets of the operand tensors.
-namespace tc {
-int tc2_launch(int bn, bool a_kmaj, bool b_kmaj, int epi, const TcOperand& A, const TcOperand& B, const TcParams& p, int kclass, cudaStream_t stream);  // gemm_tc2.cu
-}
-// CTA-pair engine selection (rlx_set_tc_pair): 0 = single-CTA kernels only; 1 = weight-gradient GEMMs on CTA pairs; 2 = every large GEMM.
-static int g_tc_pair = 2;  // measured (gpurun_out/r2_bench5_*): ms/step 98.7 (0) / 94.3 (1) / 93.3 (2, 128-wide) / 94.7 (2, 256-wide)
-bool g_tc_pair_force = false;        // test hook (rlx_debug_gemm_f32): run the pair kernel even when the problem is smaller than the machine
-static int g_tc_pair_fwd_bn = 128;  // pair tile width for the forward / dX GEMMs in mode 2 (128: double-buffered accumulators, 256: single)
-int tc_pair_mode() { return g_tc_pair; }
-int tc_pair_fwd_bn() { return g_tc_pair >= 2 ? g_tc_pair_fwd_bn : 0; }
-
-int tc_gemm_t(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int kclass, long long a_rows, long long b_rows, int n_main,
-              float* extra_col, long long extra_batch_off, long long extra_split_off, cudaStream_t stream, int transpose_out, int m_main, int pair_bn);
-
 int tc_gemm(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int kclass, long long a_rows, long long b_rows, int n_main,
-            float* extra_col, long long extra_batch_off, long long extra_split_off, cudaStream_t stream, int pair_bn) {
-  return tc_gemm_t(g, a_kmaj, b_kmaj, epi, batch, kclass, a_rows, b_rows, n_main, extra_col, extra_batch_off, extra_split_off, stream, 0, 0, pair_bn);
+            float* extra_col, long long extra_batch_off, long long extra_split_off, cudaStream_t stream) {
+  return tc_gemm_t(g, a_kmaj, b_kmaj, epi, batch, kclass, a_rows, b_rows, n_main, extra_col, extra_batch_off, extra_split_off, stream, 0, 0);
 }
 
 int tc_gemm_t(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int kclass, long long a_rows, long long b_rows, int n_main,
-              float* extra_col, long long extra_batch_off, long long extra_split_off, cudaStream_t stream, int transpose_out, int m_main, int pair_bn) {
+              float* extra_col, long long extra_batch_off, long long extra_split_off, cudaStream_t stream, int transpose_out, int m_main) {
   if (g.M <= 0 || g.N <= 0) return RLX_OK;
   if (!aligned16(g.A) || !aligned16(g.B) || !aligned16(g.C) || g.lda % 4 || g.ldb % 4 || g.ldc % 4) return RLX_ERR_UNSUPPORTED;
   if (g.splits > 1 && g.kchunk % BK) return RLX_ERR_UNSUPPORTED;
@@ -401,7 +314,7 @@ int tc_gemm_t(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int 
         gb.sA = gb.sB = gb.sC = gb.sBias = gb.sAux = 0;
         const long long ar = a_rows, br = b_kmaj ? (long long)g.N : (long long)g.K;
         const int rc = tc_gemm_t(gb, a_kmaj, b_kmaj, epi, 1, kclass, ar, br, n_main, extra_col ? extra_col + b * extra_batch_off : nullptr, 0, extra_split_off, stream,
-                                 transpose_out, m_main, pair_bn);
+                                 transpose_out, m_main);
         if (rc) return rc;
       }
       return RLX_OK;
@@ -433,48 +346,19 @@ int tc_gemm_t(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int 
               a_kmaj ? (long long)(p.a_k_off * (batch - 1) + g.K) : (long long)(p.a_mn_off * (batch - 1) + g.M), g.lda};
   TcOperand B{g.B, (b_kmaj ? (long long)p.b_mn_off : (long long)p.b_k_off) * (batch - 1) + b_rows,
               b_kmaj ? (long long)(p.b_k_off * (batch - 1) + g.K) : (long long)(p.b_mn_off * (batch - 1) + g.N), g.ldb};
-  // CTA-pair engine (gemm_tc2.cu) when the caller asked for it and the problem fills the pairs at least once
-  if (pair_bn == 128 || pair_bn == 192 || pair_bn == 256) {
-    const long long ptiles = ceil_div(g.M, 256) * ceil_div(g.N, pair_bn) * batch * g.splits;
-    if (ptiles >= sm_count() / 4 || g_tc_pair_force) {
-      const int rc = tc::tc2_launch(pair_bn, a_kmaj, b_kmaj, epi, A, B, p, kclass, stream);
-      if (rc != RLX_ERR_UNSUPPORTED) return rc;
-    }
-  }
-  // BN = 256 halves the A-operand re-reads but has a single accumulator set (no epilogue/mainloop overlap): it only pays for
-  // long reductions with a trivial epilogue (the dW GEMMs).  Short-K GEMMs with tanh / tanh' epilogues use the double-buffered
-  // BN = 128 configuration (measured: profiles/r01_tc_minibatch_ncu_details_v1.txt).
-  const long long tiles256 = ceil_div(g.M, BM) * ceil_div(g.N, 256) * batch * g.splits;
-  const int k_per_tile = (g.splits > 1) ? g.kchunk : g.K;
-  const bool use256 = (g.N % 256 == 0) && epi == TC_EPI_NONE && k_per_tile >= 256 && tiles256 >= sm_count() / 2;
-#define RLX_TC_DISPATCH(BN_)                                                                                                   \
-  do {                                                                                                                        \
-    if (p.bf16 && a_kmaj && b_kmaj && epi == TC_EPI_BIAS_TANH) return launch_cfg<BN_, true, true, TC_EPI_BIAS_TANH, true>(A, B, p, kclass, stream); \
-    if (p.bf16 && a_kmaj && !b_kmaj && epi == TC_EPI_DTANH) return launch_cfg<BN_, true, false, TC_EPI_DTANH, true>(A, B, p, kclass, stream);     \
-    if (p.bf16 && !a_kmaj && !b_kmaj && epi == TC_EPI_NONE) return launch_cfg<BN_, false, false, TC_EPI_NONE, true>(A, B, p, kclass, stream);     \
-    if (p.bf16) return RLX_ERR_UNSUPPORTED;                                                                                   \
-    if (a_kmaj && b_kmaj && epi == TC_EPI_BIAS_TANH) return launch_cfg<BN_, true, true, TC_EPI_BIAS_TANH>(A, B, p, kclass, stream); \
-    if (a_kmaj && b_kmaj && epi == TC_EPI_NONE) return launch_cfg<BN_, true, true, TC_EPI_NONE>(A, B, p, kclass, stream);       \
-    if (a_kmaj && b_kmaj && epi == TC_EPI_BIAS_RELU) return launch_cfg<BN_, true, true, TC_EPI_BIAS_RELU>(A, B, p, kclass, stream); \
-    if (a_kmaj && b_kmaj && epi == TC_EPI_BIAS) return launch_cfg<BN_, true, true, TC_EPI_BIAS>(A, B, p, kclass, stream);       \
-    if (a_kmaj && !b_kmaj && epi == TC_EPI_DRELU) return launch_cfg<BN_, true, false, TC_EPI_DRELU>(A, B, p, kclass, stream);   \
-    if (a_kmaj && !b_kmaj && epi == TC_EPI_DTANH) return launch_cfg<BN_, true, false, TC_EPI_DTANH>(A, B, p, kclass, stream);   \
-    if (a_kmaj && !b_kmaj && epi == TC_EPI_NONE) return launch_cfg<BN_, true, false, TC_EPI_NONE>(A, B, p, kclass, stream);     \
-    if (!a_kmaj && !b_kmaj && epi == TC_EPI_NONE) return launch_cfg<BN_, false, false, TC_EPI_NONE>(A, B, p, kclass, stream);   \
-  } while (0)
-  if (use256) {
-    RLX_TC_DISPATCH(256);
-  } else {
-    RLX_TC_DISPATCH(128);
-  }
-#undef RLX_TC_DISPATCH
+  if (p.bf16 && a_kmaj && b_kmaj && epi == TC_EPI_BIAS_TANH) return launch_cfg<true, true, TC_EPI_BIAS_TANH, true>(A, B, p, kclass, stream);
+  if (p.bf16 && a_kmaj && !b_kmaj && epi == TC_EPI_DTANH) return launch_cfg<true, false, TC_EPI_DTANH, true>(A, B, p, kclass, stream);
+  if (p.bf16 && !a_kmaj && !b_kmaj && epi == TC_EPI_NONE) return launch_cfg<false, false, TC_EPI_NONE, true>(A, B, p, kclass, stream);
+  if (p.bf16) return RLX_ERR_UNSUPPORTED;
+  if (a_kmaj && b_kmaj && epi == TC_EPI_BIAS_TANH) return launch_cfg<true, true, TC_EPI_BIAS_TANH>(A, B, p, kclass, stream);
+  if (a_kmaj && b_kmaj && epi == TC_EPI_NONE) return launch_cfg<true, true, TC_EPI_NONE>(A, B, p, kclass, stream);
+  if (a_kmaj && b_kmaj && epi == TC_EPI_BIAS_RELU) return launch_cfg<true, true, TC_EPI_BIAS_RELU>(A, B, p, kclass, stream);
+  if (a_kmaj && b_kmaj && epi == TC_EPI_BIAS) return launch_cfg<true, true, TC_EPI_BIAS>(A, B, p, kclass, stream);
+  if (a_kmaj && !b_kmaj && epi == TC_EPI_DRELU) return launch_cfg<true, false, TC_EPI_DRELU>(A, B, p, kclass, stream);
+  if (a_kmaj && !b_kmaj && epi == TC_EPI_DTANH) return launch_cfg<true, false, TC_EPI_DTANH>(A, B, p, kclass, stream);
+  if (a_kmaj && !b_kmaj && epi == TC_EPI_NONE) return launch_cfg<true, false, TC_EPI_NONE>(A, B, p, kclass, stream);
+  if (!a_kmaj && !b_kmaj && epi == TC_EPI_NONE) return launch_cfg<false, false, TC_EPI_NONE>(A, B, p, kclass, stream);
   return RLX_ERR_UNSUPPORTED;
 }
 
 }  // namespace rlx
-
-extern "C" int rlx_set_tc_pair(int mode, int fwd_bn) {
-  if (mode >= 0 && mode <= 2) rlx::g_tc_pair = mode;
-  if (fwd_bn == 128 || fwd_bn == 256) rlx::g_tc_pair_fwd_bn = fwd_bn;
-  return rlx::g_tc_pair;
-}

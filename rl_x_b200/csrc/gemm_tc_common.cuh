@@ -1,5 +1,5 @@
-// Shared pieces of the tcgen05 GEMM engines (gemm_tc.cu: one CTA per tile, gemm_tc2.cu: CTA pairs with cta_group::2): tile constants,
-// kernel parameters, PTX wrappers, UMMA descriptors, TMA tensor maps.
+// Pieces of the Hopper tensor-core GEMM engine (gemm_tc.cu): tile constants, kernel parameters, PTX wrappers (mbarrier, TMA,
+// wgmma), shared-memory matrix descriptors, TMA tensor maps.
 #pragma once
 #include <cuda.h>
 
@@ -9,11 +9,11 @@
 namespace rlx {
 namespace tc {
 
-constexpr int BM = 128;        // UMMA M (cta_group::1)
+constexpr int BM = 128;        // two consumer warpgroups, 64 rows each (wgmma M = 64)
+constexpr int BN = 128;        // wgmma N
 constexpr int BK = 32;         // fp32 elements per k-block = one 128-byte swizzle row
-constexpr int UMMA_K = 8;      // tf32: 32 bytes of K per instruction
-constexpr int NUM_THREADS = 448;
-constexpr int SPLIT_WARP0 = 2, EPI_WARP0 = 6, EPI_WARPS = 8;  // two epilogue warp-groups: group g takes column chunks g, g+2, ...
+constexpr int WG_K = 8;        // tf32: 32 bytes of K per wgmma
+constexpr int NUM_THREADS = 384;  // warpgroup 0: TMA + hi/lo converter; warpgroups 1, 2: wgmma consumers + epilogue
 
 enum TcEpi { TC_EPI_NONE = 0, TC_EPI_BIAS_TANH = 1, TC_EPI_DTANH = 2, TC_EPI_BIAS_RELU = 3, TC_EPI_DRELU = 4, TC_EPI_BIAS = 5 };
 
@@ -64,76 +64,60 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* bar, void* smem, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(smem)),
                "l"((uint64_t)map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
                : "memory");
 }
-// pull a box into L2 ahead of time (no shared memory, no barrier): hides DRAM latency that the 2-3 stage smem ring cannot
-__device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* map, int c0, int c1) {
-  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global [%0, {%1, %2}];" ::"l"((uint64_t)map), "r"(c0), "r"(c1) : "memory");
-}
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)map) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(cols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// wgmma shared-memory matrix descriptor (sm_90 layout): [0,14) start address >> 4, [16,30) leading byte offset >> 4,
+// [32,46) stride byte offset >> 4, [62,64) layout type (1 = SWIZZLE_128B).  Only K-major operands exist for tf32: a row of
+// 32 fp32 k-values is one 128-byte swizzle row, 8 rows form a 1024-byte atom (SBO), LBO is unused.
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr >> 4) & 0x3FFFu);
+  d |= (uint64_t)1u << 16;
+  d |= (uint64_t)(1024u >> 4) << 32;
+  d |= 1ull << 62;
+  return d;
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols) : "memory");
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accesses of accumulator registers across wgmma issue / wait
+__device__ __forceinline__ void fence_acc(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], TF32 inputs, FP32 accumulate
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+
+// D[64 x 128] (+)= A[64 x 8] * B[128 x 8]^T, both tf32 K-major in shared memory, fp32 accumulators in registers
+__device__ __forceinline__ void wgmma_tf32_m64n128k8(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-        "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]),
-        "=r"(r[31])
-      : "r"(taddr)
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),
+        "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),
+        "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
+        "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate)
       : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// UMMA shared-memory matrix descriptor, SWIZZLE_128B (cute::UMMA::SmemDescriptor bit layout):
-//   [0,14) start address >> 4   [16,30) leading byte offset >> 4   [32,46) stride byte offset >> 4   [46,48) version = 1
-//   [61,64) layout type = 2 (SWIZZLE_128B)
-//   K-major operands use SWIZZLE_128B (type 2: 16-byte chunks XOR row%8, 8-row groups of 1024 B).  MN-major 32-bit operands
-//   must use SWIZZLE_128B_BASE32B (type 1: 32-byte chunks XOR row%4, 4-row groups of 512 B) — the only MN-major layout the
-//   tensor core accepts for tf32 (cutlass sm100_common.inl:92); TMA writes it with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B.
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout_type) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFFu);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= 1ull << 46;
-  d |= (uint64_t)layout_type << 61;
-  return d;
-}
-// Instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 = 1 @ [4,6); a/b format TF32 = 2 @ [7,10) / [10,13);
-// a_major @ 15, b_major @ 16 (0 = K-major, 1 = MN-major); N >> 3 @ [17,23); M >> 4 @ [24,29)
-__host__ __device__ constexpr uint32_t make_idesc(int n, bool a_mn, bool b_mn, int m = BM) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16) | ((uint32_t)(n >> 3) << 17) |
-         ((uint32_t)(m >> 4) << 24);
 }
 
 
@@ -155,10 +139,10 @@ static inline EncodeTiledFn get_encode_fn() {
 }
 
 // 2-D fp32 row-major tensor [rows, cols] with row pitch ld (elements); box = [box_cols (<= 32), box_rows], SWIZZLE_128B.
-static inline int make_tmap(CUtensorMap* map, const float* base, long long rows, long long cols, long long ld, int box_cols, int box_rows, bool kmaj) {
+static inline int make_tmap(CUtensorMap* map, const float* base, long long rows, long long cols, long long ld, int box_cols, int box_rows) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) {
-    set_error("tcgen05 engine: cuTensorMapEncodeTiled is unavailable");
+    set_error("tensor-core engine: cuTensorMapEncodeTiled is unavailable");
     return RLX_ERR_UNSUPPORTED;
   }
   cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
@@ -166,10 +150,9 @@ static inline int make_tmap(CUtensorMap* map, const float* base, long long rows,
   cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  kmaj ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
-    set_error("tcgen05 engine: cuTensorMapEncodeTiled failed (%d) rows=%lld cols=%lld ld=%lld box=%dx%d", (int)r, rows, cols, ld, box_cols, box_rows);
+    set_error("tensor-core engine: cuTensorMapEncodeTiled failed (%d) rows=%lld cols=%lld ld=%lld box=%dx%d", (int)r, rows, cols, ld, box_cols, box_rows);
     return RLX_ERR_CUDA;
   }
   return RLX_OK;

@@ -46,7 +46,7 @@ int sm_count() {
   if (n == 0) {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;  // B200
+      n = 132;  // H100 SXM
   }
   return n;
 }

@@ -18,7 +18,6 @@
 namespace rlx {
 
 static bool use_tc(const rlx_ppo_dims& d) { return g_gemm_engine == 1 && tc_supported(d); }
-extern bool g_tc_pair_force;  // gemm_tc.cu
 }  // namespace rlx
 // comm.cu: all-reduce of [gradient | metrics]; *nblk_out > 0 when the kernel also wrote that many (policy, critic) sum-of-squares partial pairs
 int comm_allreduce_ppo(rlx_comm* c, float* out, int64_t n, const rlx_ppo_dims& d, float* norm_partials, long long* step_count, void* stream, int* nblk_out);
@@ -28,17 +27,15 @@ struct Splits {
   int splits, kchunk;
 };
 // choose a split-K factor for a [M' x N'] output reduced over `rows`: ~2 CTAs per SM for the SIMT engine, one persistent
-// CTA per SM for the tcgen05 engine (k-chunks are multiples of 32 there: one 128-byte swizzle row of fp32)
-// pair_bn > 0: the GEMM runs on CTA pairs (256 x pair_bn tiles, sm_count / 2 pairs)
-static Splits choose_splits(long long rows, int out_m, int out_n, int batch, bool tc, int pair_bn = 0) {
+// CTA per SM for the wgmma engine (k-chunks are multiples of 32 there: one 128-byte swizzle row of fp32)
+static Splits choose_splits(long long rows, int out_m, int out_n, int batch, bool tc) {
   if (tc) {
-    // persistent kernel, one CTA per SM: pick the split count whose tile total fills whole waves of SMs.  The tensor core accumulates
-    // with round-toward-zero, so each TMEM accumulation chain is also kept <= 1024 rows (128 MMAs); the long part of the
-    // reduction happens in the fp32 grad_reduce kernel (profiles/tc_accuracy_probe.py).
-    const int bn = pair_bn > 0 ? pair_bn : ((out_n % 256 == 0) ? 256 : 128);
-    const long long tiles = ceil_div(out_m, pair_bn > 0 ? 256 : 128) * ceil_div(out_n, bn) * batch;
+    // persistent kernel, one CTA per SM: pick the split count whose tile total fills whole waves of SMs.  The tensor core's
+    // accumulation error grows with the chain length, so each accumulation chain is also kept <= 1024 rows (128 MMAs); the long part
+    // of the reduction happens in the fp32 grad_reduce kernel.
+    const long long tiles = ceil_div(out_m, 128) * ceil_div(out_n, 128) * batch;
     const long long smin = std::max<long long>(1, ceil_div(rows, 1024)), smax = std::max<long long>(smin, std::min<long long>(smin + 64, rows / 64));
-    const long long sms = pair_bn > 0 ? sm_count() / 2 : sm_count();
+    const long long sms = sm_count();
     long long best = smin;
     double best_fill = -1.0;
     for (long long s = smin; s <= smax; ++s) {
@@ -103,9 +100,7 @@ static TrainPlan plan_train(const rlx_ppo_dims& d, long long m) {
   TrainPlan P;
   const long long H = d.hidden, O = d.obs_dim, A = d.act_dim;
   P.max_s1 = std::max(choose_splits(m, (int)(2 * H), (int)O, 1, false).splits, choose_splits(m, (int)O + 1, (int)(2 * H), 1, true).splits);
-  P.max_s1 = std::max(P.max_s1, choose_splits(m, (int)(2 * H), (int)O + 1, 1, true, 192).splits);  // CTA-pair orientation of dW1
   P.max_s2 = std::max(choose_splits(m, (int)H, (int)H, 2, false).splits, choose_splits(m, (int)H, (int)H, 2, true).splits);
-  P.max_s2 = std::max(P.max_s2, choose_splits(m, (int)H, (int)H, 2, true, 256).splits);
   P.head_blocks = head_grid(m);
   P.head_npart = (int)(2 * A + 5 + 2 * H);
   P.wgrad_chunks = (int)ceil_div(m, kHeadWgradRows);
@@ -160,8 +155,7 @@ static int mlp_hidden_forward(const rlx_ppo_dims& d, const PpoLayout& L, const f
   g.lda = (int)ldx; g.ldb = L.obs; g.ldc = 2 * H;
   g.splits = 1; g.kchunk = (int)(ceil_div(L.obs, 8) * 8);
   g.bf16 = bf16;
-  const int pair_fwd = tc ? tc_pair_fwd_bn() : 0;
-  int rc = run_gemm<true, true, EPI_BIAS_TANH>(tc, g, 1, stream, KC_GEMM_FWD, rows, 2 * H, pair_fwd);
+  int rc = run_gemm<true, true, EPI_BIAS_TANH>(tc, g, 1, stream, KC_GEMM_FWD, rows, 2 * H);
   if (rc) return rc;
   GemmP g2{};
   g2.A = H1; g2.B = params + L.off[W2P]; g2.C = H2; g2.bias = params + L.off[B2P];
@@ -170,7 +164,7 @@ static int mlp_hidden_forward(const rlx_ppo_dims& d, const PpoLayout& L, const f
   g2.sA = H; g2.sB = (long long)H * H; g2.sC = H; g2.sBias = H;
   g2.splits = 1; g2.kchunk = (int)(ceil_div(H, 8) * 8);
   g2.bf16 = bf16;
-  return run_gemm<true, true, EPI_BIAS_TANH>(tc, g2, 2, stream, KC_GEMM_FWD, rows, H, pair_fwd);
+  return run_gemm<true, true, EPI_BIAS_TANH>(tc, g2, 2, stream, KC_GEMM_FWD, rows, H);
 }
 
 #define RLX_DISPATCH_NCH_1(CLS, FLOPS, BYTES, KERNEL, NCH_, BF_, grid, block, smem, stream, arg)                                    \
@@ -200,9 +194,8 @@ static bool head_dims_ok(const rlx_ppo_dims& d) {
 
 int ppo_head_gemm_path(const HeadGemmArgs& a, cudaStream_t st);  // ppo_head_gemm.cu
 static int g_head_engine = 0;                                       // 0 fused SIMT kernel, 1 GEMM formulation, 2 fused mma.sync kernel (rlx_set_head_engine)
-// rlx_set_fused_tail(1): one-launch optimiser tail inside the epoch call.  Measured on B200 (round 2, gpurun_out/r2_bench3.json): SLOWER than the
-// three separate kernels (57 us vs 20 + 9 + 8 us per minibatch) - the <= SM-count grid that the grid barrier needs leaves too few threads
-// in flight for the split-K partial reads (25 MB per minibatch), which the 1287-CTA grad_reduce grid hides.  Kept as an opt-in.
+// rlx_set_fused_tail(1): one-launch optimiser tail inside the epoch call.  Off by default: the <= SM-count grid that the grid barrier needs
+// leaves few threads in flight for the split-K partial reads (25 MB per minibatch), which the much larger grad_reduce grid hides.
 static int g_fused_tail = 0;
 
 static void fill_head_common(HeadP& h, const PpoLayout& L, const float* params, const float* H2, long long rows) {
@@ -532,8 +525,7 @@ static int minibatch_fwdbwd(const rlx_ppo_minibatch_args* a, void* stream, GradR
       w3_nsplit = wgrad_chunks;
     }
     // ---- dW2 : part2[split][net][o][i] = sum_rows dZ2[r, net*H+o] * H1[r, net*H+i]   (db2 comes from the head kernel)
-    const int pair_dw = (tc && tc_pair_mode() >= 1 && H % 256 == 0) ? 256 : 0;
-    const Splits S2 = choose_splits(m, H, H, 2, tc, pair_dw);
+    const Splits S2 = choose_splits(m, H, H, 2, tc);
     s2 = S2.splits;
     GemmP g{};
     g.A = dZ2; g.B = H1; g.C = part2;
@@ -542,7 +534,7 @@ static int minibatch_fwdbwd(const rlx_ppo_minibatch_args* a, void* stream, GradR
     g.sA = H; g.sB = H; g.sC = (long long)H * H;
     g.splits = S2.splits; g.kchunk = S2.kchunk; g.sSplitC = 2LL * H * H;
     g.bf16 = bf16;
-    rc = run_gemm<false, false, EPI_NONE>(tc, g, 2, st, KC_GEMM_DW, m, m, pair_dw);
+    rc = run_gemm<false, false, EPI_NONE>(tc, g, 2, st, KC_GEMM_DW, m, m);
     if (rc) return rc;
     // ---- dZ1 = (dZ2 @ W2) * (1 - H1^2)   per net
     GemmP gd{};
@@ -552,7 +544,7 @@ static int minibatch_fwdbwd(const rlx_ppo_minibatch_args* a, void* stream, GradR
     gd.lda = 2 * H; gd.ldb = H; gd.ldc = 2 * H; gd.ldaux = 2 * H;
     gd.sA = H; gd.sB = (long long)H * H; gd.sC = H; gd.sAux = H;
     gd.splits = 1; gd.kchunk = (int)(ceil_div(H, 8) * 8);
-    rc = run_gemm<true, false, EPI_DTANH>(tc, gd, 2, st, KC_GEMM_DX, m, H, tc ? tc_pair_fwd_bn() : 0);
+    rc = run_gemm<true, false, EPI_DTANH>(tc, gd, 2, st, KC_GEMM_DX, m, H);
     if (rc) return rc;
     // ---- dW1cat | db1cat : part1[split][o][i] = sum_rows dZ1[r, o] * X[r, i];  db1[o] = sum_rows dZ1[r, o]
     GemmP g1{};
@@ -561,24 +553,9 @@ static int minibatch_fwdbwd(const rlx_ppo_minibatch_args* a, void* stream, GradR
     g1.M = 2 * H; g1.N = O; g1.K = (int)m;
     g1.lda = 2 * H; g1.ldb = (int)ldx; g1.ldc = O;
     bool done = false;
-    if (tc && a->states_ones_col && tc_pair_mode() >= 1 && (2 * H) % 256 == 0) {
-      // CTA pairs, NOT transposed: M = 2H (whole 256-row pair tiles), N = O + 1 in 192-wide tiles (377 -> 2 x 192); the constant-one
-      // column of X lands in output column O, which the epilogue diverts into rs1 (= db1)
-      const Splits S1 = choose_splits(m, 2 * H, O + 1, 1, true, 192);
-      GemmP gp = g1;
-      gp.N = O + 1;
-      gp.splits = S1.splits; gp.kchunk = S1.kchunk; gp.sSplitC = 2LL * H * O;
-      rc = tc_gemm(gp, false, false, TC_NONE, 1, KC_GEMM_DW, m, m, O, rs1, 0, 2LL * H, st, 192);
-      if (rc == RLX_OK) {
-        done = true;
-        s1 = S1.splits;
-      } else if (rc != RLX_ERR_UNSUPPORTED) {
-        return rc;
-      }
-    }
-    if (!done && tc && a->states_ones_col) {
+    if (tc && a->states_ones_col) {
       // tensor-core path, computed TRANSPOSED: C^T[i, o] = sum_r X_aug[r, i] dZ1[r, o] with M = O+1 (the constant-one column of X
-      // makes db1 the last output row) and N = 2H = full 256-wide tiles; the epilogue stores C^T transposed back into [o][i].
+      // makes db1 the last output row) and N = 2H = whole 128-wide tiles; the epilogue stores C^T transposed back into [o][i].
       const Splits S1 = choose_splits(m, O + 1, 2 * H, 1, true);
       GemmP gt{};
       gt.A = states; gt.B = dZ1; gt.C = part1;
@@ -806,6 +783,7 @@ extern "C" int rlx_debug_gemm_f32(int engine, int layout, int epilogue, int64_t 
                                   const float* B, int64_t ldb, float* C, int64_t ldc, const float* bias, const float* aux, int64_t ldaux,
                                   void* stream) {
   RLX_CHECK_ARG(A && B && C && M > 0 && N > 0 && K > 0, "bad arguments");
+  RLX_CHECK_ARG(engine == 0 || engine == 1, "unknown engine (0 = SIMT, 1 = wgmma tensor cores)");
   RLX_CHECK_ARG((epilogue == 0) || (epilogue == 1 && layout == 0 && bias) || (epilogue == 2 && layout == 1 && aux), "unsupported epilogue/layout");
   GemmP g{};
   g.A = A; g.B = B; g.C = C; g.bias = bias; g.aux = aux;
@@ -815,13 +793,9 @@ extern "C" int rlx_debug_gemm_f32(int engine, int layout, int epilogue, int64_t 
   cudaStream_t st = (cudaStream_t)stream;
   const bool a_k = layout != 2, b_k = layout == 0;
   const long long a_rows = a_k ? M : K, b_rows = b_k ? N : K;
-  if (engine >= 1 && engine <= 4) {
-    // 1: single-CTA tcgen05 kernels; 2 / 3 / 4: CTA-pair kernels (cta_group::2) with 128 / 256 / 192-wide tiles
-    const int pair_bn = engine == 2 ? 128 : engine == 3 ? 256 : engine == 4 ? 192 : 0;
-    g_tc_pair_force = pair_bn != 0;
-    const int rc = tc_gemm(g, a_k, b_k, epilogue, 1, KC_OTHER, a_rows, b_rows, 0, nullptr, 0, 0, st, pair_bn);
-    g_tc_pair_force = false;
-    if (rc == RLX_ERR_UNSUPPORTED) set_error("rlx_debug_gemm_f32: shape/alignment not supported by the tcgen05 engine");
+  if (engine == 1) {
+    const int rc = tc_gemm(g, a_k, b_k, epilogue, 1, KC_OTHER, a_rows, b_rows, 0, nullptr, 0, 0, st);
+    if (rc == RLX_ERR_UNSUPPORTED) set_error("rlx_debug_gemm_f32: shape/alignment not supported by the wgmma engine");
     return rc;
   }
   if (layout == 0 && epilogue == 1) return launch_sgemm<true, true, EPI_BIAS_TANH>(g, 1, st);

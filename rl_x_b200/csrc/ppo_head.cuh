@@ -591,7 +591,7 @@ __global__ void __launch_bounds__(512) ppo_head_wgrad2_kernel(const HeadWgrad2P 
 // ------------------------------------------------------------ train head, vectorised variant (H multiple of 128)
 // Lane l owns the 4-column groups {g*128 + 4l .. +3}: H2 / dZ2 rows move as coalesced 128-bit accesses and every W3 fetch is
 // one conflict-free LDS.128 that feeds 8 FMAs (2 rows x 4 columns).  ~1.3k warp instructions per row pair (the scalar variant
-// above needs ~7k: it is issue-bound, profiles/r01_tc_minibatch_ncu_details_v1.txt).
+// above needs ~7k: it is issue-bound).
 __device__ __forceinline__ float dot4(const float4& a, const float4& b, float s) {
   s = fmaf(a.x, b.x, s); s = fmaf(a.y, b.y, s); s = fmaf(a.z, b.z, s); return fmaf(a.w, b.w, s);
 }

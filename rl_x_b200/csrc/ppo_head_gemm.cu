@@ -7,8 +7,8 @@
 //   (4) column sums (layer-2 / head bias gradients, log-std gradient, metric sums) written as ONE partial block in the fused kernel's
 //       layout, so the rest of rlx_ppo_minibatch_fwdbwd_f32 (dW3 / dW2 / dX / dW1 GEMMs, grad_reduce) is unchanged
 // moves the heavy parts onto the GEMM engines.  This file is dual-build (dual_build.cuh): its host emulation is checked against the
-// PPO oracle's autograd in tests/test_lstm_emulation.py::test_emulated_ppo_head_gemm_path.  Timed in round 2 with the exact-fp32 SIMT GEMMs:
-// slower than the fused kernel (142 vs 95 ms per iteration, DESIGN.md 4c), so it stays an opt-in.
+// PPO oracle's autograd in tests/test_lstm_emulation.py::test_emulated_ppo_head_gemm_path.  It stays an opt-in
+// (DESIGN.md 4c); the fused kernel is the default.
 #include "flat_ops.cuh"
 #include "ppo_head_gemm.cuh"
 

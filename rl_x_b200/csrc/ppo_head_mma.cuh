@@ -1,7 +1,7 @@
 // Train head on the legacy tensor path (mma.sync m16n8k8, 3xTF32): rlx_set_head_engine(2).
 //
-// The fused SIMT head (ppo_head_train3_kernel) is issue-bound: ~1.1k warp instructions per row for 2 x 256 x 18 FMAs, 80 us per
-// 32768-row minibatch against ~25 us of HBM time (profiles/r02_minibatch_ncu.txt).  Here the two skinny products
+// The fused SIMT head (ppo_head_train3_kernel) is issue-bound: ~1.1k warp instructions per row for 2 x 256 x 18 FMAs, several
+// times the HBM time of a 32768-row minibatch.  Here the two skinny products
 //     mean[M, act] = H2p[M, H] . W3p^T          and          dH2p[M, H] = dmean[M, act] . W3p
 // run as warp-level MMAs on 16-row tiles, everything else (log-prob, ratio, surrogate, value loss, tanh', bias-gradient and metric
 // partial sums) stays in the registers of the same kernel, in the same arithmetic as the SIMT head (ref: ppo.py:121-141,153-157).

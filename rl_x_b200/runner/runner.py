@@ -4,7 +4,7 @@ from the plugins' defaults + `--tree.key=value` flags, create envs, construct th
 
 absl / ml_collections / gymnasium are not in this image, so flags are parsed by rl_x_b200.config_dict.apply_overrides.
 `implementation_package_names` works as in the reference: packages are tried in order, so
-`Runner(implementation_package_names=["rl_x_b200", "rl_x"])` lets B200 plugins and reference plugins coexist."""
+`Runner(implementation_package_names=["rl_x_b200", "rl_x"])` lets this package's plugins and reference plugins coexist."""
 import importlib
 import logging
 import logging.handlers

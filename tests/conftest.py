@@ -12,12 +12,12 @@ GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box: pytest -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100: pytest -m gpu)")
 
 
 def pytest_sessionfinish(session, exitstatus):
     """RLX_AUX_ENGINE_REPORT=<file>: leave "<tensor GEMMs> <persistent recurrence launches>" of this process - the FastSAC / PPO+LSTM GEMMs
-    that ran on the tcgen05 engine and the one-launch-per-direction LSTM recurrences (the subprocess runs of run_suite_with_switches below read
+    that ran on the wgmma engine and the one-launch-per-direction LSTM recurrences (the subprocess runs of run_suite_with_switches below read
     it back: a green suite that never took the path it was asked to take proves nothing)."""
     path = os.environ.get("RLX_AUX_ENGINE_REPORT")
     if path:
@@ -32,7 +32,7 @@ def pytest_sessionfinish(session, exitstatus):
 
 
 def run_suite_with_switches(test_file, tmp_path, tensor_engine=False, persistent=False, timeout=900):
-    """Run the GPU parity tests of `test_file` again in a SUBPROCESS with the opt-in paths on: RLX_AUX_GEMM_ENGINE=1 (dense layers on the tcgen05
+    """Run the GPU parity tests of `test_file` again in a SUBPROCESS with the opt-in paths on: RLX_AUX_GEMM_ENGINE=1 (dense layers on the wgmma
     3xTF32 engine where it covers the product) and / or RLX_LSTM_PERSISTENT=1 (LSTM recurrence as one block-cooperative launch per direction).
     A subprocess because a kernel that traps or faults takes the CUDA context with it: here that costs one test, not the rest of the
     session.  Returns (returncode, output tail, tensor GEMM count, persistent launch count); the counts are -1 when no report came back."""

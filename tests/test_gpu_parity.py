@@ -19,7 +19,7 @@ pytestmark = pytest.mark.gpu
 
 @pytest.fixture(autouse=True, params=["simt", "tcgen05"])
 def gemm_engine(request):
-    """Every test runs once per GEMM engine (shapes the tcgen05 engine does not cover fall back to the SIMT engine)."""
+    """Every test runs once per GEMM engine (shapes the wgmma engine, selected as "tcgen05", does not cover fall back to the SIMT engine)."""
     from rl_x_b200 import _native as nt
     lib = nt.load()
     lib.rlx_set_gemm_engine(1 if request.param == "tcgen05" else 0)

@@ -1,4 +1,4 @@
-"""The tcgen05 3xTF32 GEMM engine in isolation (rlx_debug_gemm_f32): every operand layout / epilogue the MLP uses, with
+"""The wgmma 3xTF32 GEMM engine in isolation (rlx_debug_gemm_f32): every operand layout / epilogue the MLP uses, with
 M / N / K tails, against an fp64 reference and against the exact-fp32 SIMT engine."""
 import numpy as np
 import pytest
@@ -20,7 +20,7 @@ def _err(c, ref):
 
 CASES = [
     # layout, epilogue, M, N, K
-    (0, 0, 128, 128, 32), (0, 0, 128, 256, 64), (0, 1, 4096, 512, 376), (0, 1, 130, 256, 256), (0, 0, 1000, 128, 64), (0, 1, 32, 512, 376),
+    (0, 0, 128, 128, 32), (0, 0, 128, 256, 64), (0, 1, 4096, 512, 376), (0, 1, 40000, 512, 376), (0, 1, 130, 256, 256), (0, 0, 1000, 128, 64), (0, 1, 32, 512, 376),
     (1, 0, 256, 256, 256), (1, 2, 4100, 256, 256), (1, 2, 33, 256, 256),
     (2, 0, 128, 128, 64), (2, 0, 256, 256, 3000), (2, 0, 512, 380, 2752), (2, 0, 512, 380, 40), (2, 0, 256, 256, 5),
 ]
@@ -55,9 +55,8 @@ def test_tc_gemm_is_fp32_accurate(layout, epi, M, N, K):
         out[engine] = _err(C, ref)
     (simt_fro, simt_max), (tc_fro, tc_max) = out[0], out[1]
     assert simt_fro < 2e-6
-    # Measured error model of the 3xTF32 engine (profiles/tc_accuracy_probe.py): ~4e-7 from the split itself plus ~2.3e-9 per
-    # reduction element from the tensor core's round-toward-zero accumulation (production dW GEMMs keep chains <= 1024 via split-K).
-    # Single-pass TF32 would sit at ~5e-4 here.
+    # Error model of the 3xTF32 engine: ~4e-7 from the split itself plus a few 1e-9 per reduction element from the tensor core's
+    # accumulation rounding (production dW GEMMs keep chains <= 1024 via split-K).  Single-pass TF32 would sit at ~5e-4 here.
     bound = 6e-7 + 3.2e-9 * K
     assert tc_fro < bound, (out, bound, "3xTF32 engine is not fp32-accurate")
     assert tc_max < max(10 * bound, 4 * simt_max), (out, bound)
@@ -66,49 +65,16 @@ def test_tc_gemm_is_fp32_accurate(layout, epi, M, N, K):
 def test_tc_gemm_rejects_unaligned_shapes():
     k = _k()
     A, B, C = torch.randn(64, 30, device=DEV), torch.randn(64, 30, device=DEV), torch.empty(64, 64, device=DEV)
-    with pytest.raises(RuntimeError, match="not supported by the tcgen05 engine"):
+    with pytest.raises(RuntimeError, match="not supported by the wgmma engine"):
         k.debug_gemm(1, 0, 0, A, B, C, 64, 64, 30)
 
 
-# CTA-pair engine (cta_group::2, csrc/gemm_tc2.cu): engine 2 / 3 / 4 = 256 x 128 / 256 x 256 / 256 x 192 pair tiles.  Shapes cover: one pair
-# tile, a peer CTA whose rows are entirely out of bounds (M <= 128), ragged M / N / K, many tiles per pair (persistent loop + both
-# accumulator stages), all layouts and epilogues the MLP uses.
-PAIR_CASES = [
-    (2, 0, 0, 256, 128, 32), (2, 0, 0, 128, 128, 64), (2, 0, 1, 4096, 512, 376), (2, 0, 1, 130, 256, 256), (2, 0, 1, 40000, 512, 376),
-    (2, 1, 2, 4100, 256, 256), (2, 1, 0, 256, 256, 256), (2, 2, 0, 512, 256, 3000),
-    (3, 0, 0, 256, 256, 32), (3, 0, 1, 4096, 512, 376), (3, 0, 1, 20000, 512, 376), (3, 1, 2, 4100, 256, 256), (3, 2, 0, 256, 256, 3000), (3, 2, 0, 512, 256, 1024),
-    (3, 2, 0, 256, 256, 5),
-    (4, 2, 0, 512, 380, 2752), (4, 2, 0, 512, 377, 1024), (4, 2, 0, 256, 192, 40),
-]
-
-
-@pytest.mark.parametrize("engine,layout,epi,M,N,K", PAIR_CASES)
-def test_tc_pair_gemm_is_fp32_accurate(engine, layout, epi, M, N, K):
+@pytest.mark.parametrize("engine", [-1, 2, 3, 4])
+def test_debug_gemm_rejects_unknown_engines(engine):
+    """Engines 2-4 once selected CTA-pair kernels: an old caller must get an error, not a silent SIMT result."""
     k = _k()
-    g = torch.Generator().manual_seed(M * 7 + N * 3 + K + engine)
-    if layout == 0:
-        A, B = torch.randn(M, K, generator=g), torch.randn(N, K, generator=g) * 0.3
-        ref = A.double() @ B.double().T
-    elif layout == 1:
-        A, B = torch.randn(M, K, generator=g), torch.randn(K, N, generator=g) * 0.3
-        ref = A.double() @ B.double()
-    else:
-        ldn = -(-N // 4) * 4  # the MN-major B operand keeps a 16-byte row pitch (the gathered states: 377 valid columns, pitch 380)
-        A, B = torch.randn(K, M, generator=g), torch.randn(K, ldn, generator=g) * 0.3
-        ref = A.double().T @ B[:, :N].double()
-    bias = torch.randn(N, generator=g) if epi == 1 else None
-    aux = torch.tanh(torch.randn(M, N, generator=g)) if epi == 2 else None
-    if epi == 1:
-        ref = torch.tanh(ref + bias.double())
-    if epi == 2:
-        ref = ref * (1 - aux.double() ** 2)
-    ldc = -(-N // 4) * 4
-    C = torch.full((M, ldc), float("nan"), device=DEV)
-    k.debug_gemm(engine, layout, epi, A.to(DEV), B.to(DEV), C, M, N, K, bias=bias.to(DEV) if bias is not None else None,
-                 aux=aux.to(DEV) if aux is not None else None)
+    A, B, C = torch.randn(128, 32, device=DEV), torch.randn(128, 32, device=DEV), torch.full((128, 128), float("nan"), device=DEV)
+    with pytest.raises(RuntimeError, match="unknown engine"):
+        k.debug_gemm(engine, 0, 0, A, B, C, 128, 128, 32)
     torch.cuda.synchronize()
-    C = C[:, :N]
-    assert torch.isfinite(C).all(), "pair engine left unwritten / non-finite outputs"
-    fro, mx = _err(C, ref)
-    bound = 6e-7 + 3.2e-9 * K
-    assert fro < bound, (fro, mx, bound)
+    assert torch.isnan(C).all()

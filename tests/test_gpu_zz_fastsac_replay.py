@@ -1,7 +1,5 @@
 """FastSAC n-step replay sampling kernel (rlx_replay_sample_nstep_f32) against the executed reference (tests/golden/fastsac_replay.npz)
-and against oracle/fastsac_replay_oracle.py on a large random ring.
-
-First passed on a B200 at the round-1 driver run (GPUTEST_r01.json); strict since round 2."""
+and against oracle/fastsac_replay_oracle.py on a large random ring."""
 import numpy as np
 import pytest
 import torch

@@ -1,6 +1,5 @@
 """Opt-in GEMM formulation of the PPO loss head (rlx_set_head_engine(1), csrc/ppo_head_gemm.cu) inside rlx_ppo_minibatch_fwdbwd_f32:
-gradients and metrics must equal the default fused-kernel head's.  Host emulation of the same source: tests/test_lstm_emulation.py::test_emulated_ppo_head_gemm_path.
-First passed on a B200 at the round-1 driver run; strict since round 2."""
+gradients and metrics must equal the default fused-kernel head's.  Host emulation of the same source: tests/test_lstm_emulation.py::test_emulated_ppo_head_gemm_path."""
 import numpy as np
 import pytest
 import torch

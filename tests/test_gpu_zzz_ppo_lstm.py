@@ -1,8 +1,7 @@
 """PPO+LSTM path on the GPU (rl_x_b200/csrc/lstm.cu through librlx_b200.so) against oracle/ppo_lstm_oracle.py.
 
-The same sources are validated in host emulation (tests/test_lstm_emulation.py).  First passed on a B200 at the round-1 driver run;
-strict since round 2.  The FiLM / shared-encoder cases and the one-launch-per-step recurrence were written after the round-2 GPU budget
-was spent: they passed the emulation suite, their first hardware run is the driver's."""
+The same sources are validated in host emulation (tests/test_lstm_emulation.py), including the FiLM / shared-encoder options and the
+one-launch-per-step recurrence."""
 import ctypes as C
 import os
 
@@ -18,9 +17,6 @@ DEV = "cuda"
 
 
 OPT_FILM, OPT_SHARED = 1, 2   # RLX_LSTM_OPT_*
-# Paths whose first hardware run is the driver's (written after the round-2 GPU budget was spent; validated in host emulation only).
-# Not strict: a failure here must be visible in the report without hiding the rest of the suite behind `-x`.
-FIRST_RUN = pytest.mark.xfail(strict=False, reason="first hardware run of this path (validated in host emulation, tests/test_lstm_emulation.py)")
 
 
 def _perturbed(obs, act, hid, enc, lstm, seed, options=0):
@@ -38,9 +34,8 @@ def _perturbed(obs, act, hid, enc, lstm, seed, options=0):
 @pytest.mark.parametrize("T,n,obs,act,hid,enc,lstm,options", [
     (7, 5, 6, 2, 12, 8, 4, 0), (33, 40, 5, 2, 8, 8, 4, 0), (16, 24, 64, 8, 256, 128, 64, 0), (128, 256, 64, 8, 256, 128, 64, 0),
     # lstm_obs_combine_method = "film" / share_lstm_obs_encoder (policy.py:51-59, 99-125)
-    pytest.param(7, 5, 6, 2, 12, 8, 4, OPT_FILM, marks=FIRST_RUN), pytest.param(7, 5, 6, 2, 12, 8, 4, OPT_SHARED, marks=FIRST_RUN),
-    pytest.param(33, 40, 5, 2, 8, 8, 4, OPT_FILM | OPT_SHARED, marks=FIRST_RUN), pytest.param(16, 24, 64, 8, 256, 128, 64, OPT_FILM, marks=FIRST_RUN),
-    pytest.param(16, 24, 64, 8, 256, 128, 64, OPT_FILM | OPT_SHARED, marks=FIRST_RUN)])
+    (7, 5, 6, 2, 12, 8, 4, OPT_FILM), (7, 5, 6, 2, 12, 8, 4, OPT_SHARED), (33, 40, 5, 2, 8, 8, 4, OPT_FILM | OPT_SHARED),
+    (16, 24, 64, 8, 256, 128, 64, OPT_FILM), (16, 24, 64, 8, 256, 128, 64, OPT_FILM | OPT_SHARED)])
 def test_lstm_fwdbwd_matches_oracle_autograd(T, n, obs, act, hid, enc, lstm, options):
     from rl_x_b200 import _native as nt
     lib = nt.load()
@@ -123,7 +118,6 @@ def _plugin_run(combine="concat", share=False, graph=False, iterations=2):
     return model, logged
 
 
-@FIRST_RUN
 @pytest.mark.parametrize("combine,share", [("film", False), ("concat", True), ("film", True)])
 def test_lstm_plugin_options_train(combine, share):
     """lstm_obs_combine_method / share_lstm_obs_encoder through the plugin: finite metrics, every live parameter segment moves, the segments
@@ -138,7 +132,6 @@ def test_lstm_plugin_options_train(combine, share):
         assert float((pol[name] - pol0[name]).abs().max()) > 1e-6, name
 
 
-@FIRST_RUN
 def test_lstm_plugin_cuda_graph_replay_equals_eager_launches():
     """use_cuda_graph replays each minibatch update as one captured graph: same kernels in the same order on the same buffers, no atomics,
     so three iterations leave bit-identical weights, Adam moments and logged metrics."""
@@ -151,9 +144,8 @@ def test_lstm_plugin_cuda_graph_replay_equals_eager_launches():
     assert keep(log_e) == keep(log_r)
 
 
-@FIRST_RUN
 def test_lstm_suite_in_a_subprocess_with_dense_layers_on_the_tensor_engine(tmp_path):
-    """rlx_set_aux_gemm_engine(1): every dense layer of the update with at least half a tile per output dimension runs on the tcgen05 3xTF32
+    """rlx_set_aux_gemm_engine(1): every dense layer of the update with at least half a tile per output dimension runs on the wgmma 3xTF32
     engine (forward and input-gradient products on K-major copies of the kernels), the heads stay on the SIMT engine.  The whole file -
     oracle parity at the config-5 shape included - must pass that way, and must actually have used the tensor engine."""
     from conftest import run_suite_with_switches
@@ -162,7 +154,6 @@ def test_lstm_suite_in_a_subprocess_with_dense_layers_on_the_tensor_engine(tmp_p
     assert tc > 0, f"the tensor engine was never used ({tc})"
 
 
-@FIRST_RUN
 def test_lstm_suite_in_a_subprocess_with_the_one_launch_recurrence(tmp_path):
     """rlx_set_lstm_persistent(1): the recurrence of every update as ONE block-cooperative launch per direction (recurrent kernel in shared
     memory, a barrier per step).  Bit-identical to the per-step path in emulation (and race-free under ThreadSanitizer); on the device the

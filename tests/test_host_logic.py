@@ -333,7 +333,7 @@ def test_checkpoint_written_by_the_reference_maps_onto_the_flat_layout():
             for f in ("exp_avg", "exp_avg_sq"):
                 assert torch.equal(ours["state"][i][f], ref["state"][i][f]), (key, i, f)
             assert float(ours["state"][i]["step"]) == float(ref["state"][i]["step"])
-    # a permuted optimizer state (the round-1 bug: logstd last) is rejected instead of being mis-assigned
+    # a permuted optimizer state (logstd last, a bug of an earlier version) is rejected instead of being mis-assigned
     bad = {"state": {i: ck["policy_optimizer_state_dict"]["state"][(i + 1) % 7] for i in range(7)}}
     with pytest.raises(ValueError, match="expected"):
         fp.load_adam_state(bad, POLICY_PARAM_ORDER, nt.POLICY_KEYS, m1, m2)
@@ -468,40 +468,6 @@ def test_build_digest_does_not_depend_on_the_checkout_path(tmp_path, monkeypatch
     with open(other / "csrc" / "gae.cu", "a") as fh:
         fh.write("\n// changed\n")
     assert b._digest() != here
-
-
-def _last_json_line(path):
-    import json
-    with open(path) as fh:
-        lines = [ln for ln in fh.read().splitlines() if ln.startswith("{")]
-    return json.loads(lines[-1])
-
-
-def test_committed_bench_records_carry_the_contract_keys():
-    """The bench lines committed under profiles/ (the last hardware runs of `python bench.py` and `bench.py --impl reference`) against the
-    key list of the measurement contract: a renamed or dropped key would otherwise only be noticed by the driver."""
-    import os
-    prof = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "profiles")
-    line = _last_json_line(os.path.join(prof, "r02_bench_1gpu.json"))
-    for key in ["metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline", "dtype", "data",
-                "config", "gpu_launches", "clocks", "roofline", "cpu_baseline", "e2e"]:
-        assert key in line, key
-    assert line["n_gpus"] == 1 and line["warmup"] >= 3 and line["higher_is_better"] is True and line["vs_baseline"] is None
-    assert line["dtype"] == "f32" and line["data"] == "synthetic" and "workload" in line["config"] and "model" not in line["config"]
-    assert abs(line["value"] - 4096 * 128 / (line["ms_per_step"] * 1e-3)) <= 1e-6 * line["value"]       # value and ms_per_step tell one story
-    roof = line["roofline"]
-    assert set(["bound", "achieved", "peak", "unit", "frac", "traffic"]) <= set(roof) and roof["bound"] in ("hbm", "tensor")
-    assert abs(roof["frac"] - roof["achieved"] / roof["peak"]) <= 1e-9
-    assert set(["value", "unit", "cores", "kind", "sample"]) <= set(line["cpu_baseline"]) and line["cpu_baseline"]["kind"] in ("reference", "port")
-    e2e = line["e2e"]
-    assert set(["value", "unit", "h2d_bytes_per_step", "d2h_bytes_per_step"]) <= set(e2e) and e2e["h2d_bytes_per_step"] > 0 < e2e["d2h_bytes_per_step"]
-    assert e2e["value"] < line["value"]                              # host copies inside the timed region cannot be free
-    assert set(["sm_mhz", "sm_max_mhz", "reasons"]) <= set(line["clocks"]) and line["gpu_launches"] > 0
-    assert not set(line["clocks"]["reasons"]) & {"hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown"}
-    ref = _last_json_line(os.path.join(prof, "r02_reference_arm.json"))
-    assert ref["impl"] == "reference" and ref["metric"] == line["metric"] and ref["unit"] == line["unit"] and ref["config"]["workload"] == line["config"]["workload"]
-    assert ref["e2e"]["h2d_bytes_per_step"] == 0 == ref["e2e"]["d2h_bytes_per_step"] and ref["e2e"]["value"] == ref["value"]
-    assert ref["cpu_baseline"]["kind"] == "reference" and ref["cpu_baseline"]["value"] == ref["value"]
 
 
 def test_sac_checkpoint_written_by_the_reference_maps_onto_the_flat_layout():
@@ -748,41 +714,33 @@ def test_importing_a_plugin_package_registers_it_with_the_reference_too():
         assert ref_environments.get_environment_general_properties(name).action_space_type.name == "CONTINUOUS"
 
 
+def _reference_surface():
+    """Default configs and model-class method signatures of the reference's five algorithms (tests/golden/make_golden_reference_surface.py)."""
+    import json
+    with open(os.path.join(ROOT, "tests", "golden", "reference_surface.json")) as fh:
+        return json.load(fh)
+
+
 def test_default_configs_carry_every_reference_key_with_the_reference_value():
     """Every key of the reference's default_config.py of the five algorithms is present with the SAME default, except the one documented
-    difference (bf16_mixed_precision_training: this build's default is the fp32 parity path); keys this build adds are not reference keys.
-    Reference modules: the staged copies (ppo, sac, fastsac) and, in the build container only, /root/reference for espo and ppo_lstm."""
+    difference (bf16_mixed_precision_training: this build's default is the fp32 parity path); keys this build adds are not reference keys."""
     import importlib
-    import runpy
-    from oracle import make_ref, ref_arm
-    if not make_ref.available():
-        pytest.skip("oracle/_ref not staged (python oracle/make_ref.py)")
-    ref_arm._install_stub()
-    sources = {"ppo": os.path.join(make_ref.DST, "rl_x/algorithms/ppo/pytorch/default_config.py"),
-               "sac": os.path.join(make_ref.DST, "rl_x/algorithms/sac/pytorch/default_config.py"),
-               "fastsac": os.path.join(make_ref.DST, "rl_x/algorithms/fastsac/pytorch/default_config.py"),
-               "espo": "/root/reference/rl_x/algorithms/espo/pytorch/default_config.py",
-               "ppo_lstm": "/root/reference/rl_x/algorithms/ppo_lstm/flax/default_config.py"}
-    checked = 0
-    for algo, path in sources.items():
-        if not os.path.exists(path):
-            continue
-        ref = runpy.run_path(path)["get_config"]("x")
-        ours = importlib.import_module(f"rl_x_b200.algorithms.{algo}.b200.default_config").get_config("x")
+    import json
+    surface = _reference_surface()
+    assert sorted(surface) == ["espo", "fastsac", "ppo", "ppo_lstm", "sac"]
+    for algo, entry in surface.items():
+        ref = entry["config"]
+        cfg = importlib.import_module(f"rl_x_b200.algorithms.{algo}.b200.default_config").get_config("x")
+        ours = {k: json.loads(json.dumps(cfg[k])) for k in cfg}   # same normal form as the stored values (tuples -> lists)
         assert [k for k in ref if k not in ours] == [], algo
         different = {k: (ref[k], ours[k]) for k in ref if k != "name" and ref[k] != ours[k]}
         assert set(different) <= {"bf16_mixed_precision_training"}, (algo, different)
-        checked += 1
-    assert checked >= 3
 
 
 def test_model_classes_have_the_reference_classes_methods_and_signatures():
     """Duck typing is the boundary (SURVEY 8 b): every method of the reference's model class exists on this package's class with the same
     parameter names (`load` may be a classmethod: the runner calls it on the class either way, runner.py:334-337).  Read from the sources."""
     import ast
-    from oracle import make_ref
-    if not make_ref.available():
-        pytest.skip("oracle/_ref not staged (python oracle/make_ref.py)")
 
     def methods(path, cls):
         for node in ast.walk(ast.parse(open(path).read())):
@@ -791,19 +749,15 @@ def test_model_classes_have_the_reference_classes_methods_and_signatures():
         raise AssertionError(f"no class {cls} in {path}")
 
     pkg = os.path.join(ROOT, "rl_x_b200", "algorithms")
-    cases = [("PPO", os.path.join(make_ref.DST, "rl_x/algorithms/ppo/pytorch/ppo.py"), [f"{pkg}/ppo/b200/ppo.py"]),
-             ("SAC", os.path.join(make_ref.DST, "rl_x/algorithms/sac/pytorch/sac.py"), [f"{pkg}/sac/b200/sac.py"]),
-             ("FastSAC", os.path.join(make_ref.DST, "rl_x/algorithms/fastsac/pytorch/fastsac.py"), [f"{pkg}/fastsac/b200/fastsac.py"]),
-             ("ESPO", "/root/reference/rl_x/algorithms/espo/pytorch/espo.py", [f"{pkg}/ppo/b200/ppo.py", f"{pkg}/espo/b200/espo.py"]),
-             ("PPO_LSTM", "/root/reference/rl_x/algorithms/ppo_lstm/flax/ppo_lstm.py", [f"{pkg}/ppo_lstm/b200/ppo_lstm.py"])]
-    checked = 0
-    for cls, ref_path, our_paths in cases:
-        if not os.path.exists(ref_path):
-            continue
-        ref, ours = methods(ref_path, cls), {}
-        for p, c in zip(our_paths, ["PPO", cls] if len(our_paths) == 2 else [cls]):   # ESPO inherits PPO here
-            ours.update(methods(p, c))
-        assert [m for m in ref if m not in ours] == [], cls
-        assert {m: (ref[m], ours[m]) for m in ref if ref[m] != ours[m]} == {}, cls
-        checked += 1
-    assert checked >= 3
+    ours_of = {"ppo": [("PPO", f"{pkg}/ppo/b200/ppo.py")], "sac": [("SAC", f"{pkg}/sac/b200/sac.py")],
+               "fastsac": [("FastSAC", f"{pkg}/fastsac/b200/fastsac.py")],
+               "espo": [("PPO", f"{pkg}/ppo/b200/ppo.py"), ("ESPO", f"{pkg}/espo/b200/espo.py")],   # ESPO inherits PPO here
+               "ppo_lstm": [("PPO_LSTM", f"{pkg}/ppo_lstm/b200/ppo_lstm.py")]}
+    surface = _reference_surface()
+    assert sorted(surface) == sorted(ours_of)
+    for algo, entry in surface.items():
+        ref, ours = entry["methods"], {}
+        for cls, path in ours_of[algo]:
+            ours.update(methods(path, cls))
+        assert [m for m in ref if m not in ours] == [], entry["class"]
+        assert {m: (ref[m], ours[m]) for m in ref if ref[m] != ours[m]} == {}, entry["class"]

@@ -89,7 +89,7 @@ def _np(t):
 @pytest.mark.parametrize("T,n,obs,act,hid,enc,lstm", [
     (7, 5, 6, 2, 12, 8, 4), (5, 3, 9, 3, 16, 12, 8), (33, 40, 5, 2, 8, 8, 4),
     # BASELINE config 5's minibatch (128 steps x 256 envs, reference widths): ~2 min per option set with RLX_EMU_CXXFLAGS=-O2, so on request
-    # only.  Last run (round 2, all four option sets): worst entry at 0.3 % of the GPU test's tolerance.
+    # only.
     pytest.param(128, 256, 64, 8, 256, 128, 64, marks=pytest.mark.skipif(os.environ.get("RLX_SLOW_TESTS") != "1", reason="slow: RLX_SLOW_TESTS=1"))])
 def test_emulated_lstm_fwdbwd_matches_oracle_autograd(emu, T, n, obs, act, hid, enc, lstm, options):
     torch.manual_seed(T * 100 + n)
