@@ -291,10 +291,6 @@ int rlx_set_head_engine(int engine);
  * the reference.  bf16 values are exact TF32 operands, so the tensor-core GEMMs run ONE tf32 wgmma per product in this mode (fp32
  * accumulation, as a bf16 tensor-core GEMM accumulates) instead of the three of the fp32-equivalent split.  Returns the setting. */
 int rlx_set_autocast_bf16(int on);
-/* 1: rlx_ppo_update_epoch_f32 runs gradient assembly + both grad norms + clip + Adam of a minibatch as ONE kernel (grid barrier in the
- * caller's workspace); 0 (default): the three separate kernels of rlx_ppo_minibatch_fwdbwd_f32 /
- * rlx_gradnorm_clip_adam_f32.  Returns the setting. */
-int rlx_set_fused_tail(int on);
 /* bring-up / test entry of the GEMM head on caller buffers: H2 [m, 2*hidden] (policy | critic halves), torch-layout head weights; outputs
  * dZ2 [m, 2*hidden], dhead [m, round_up(act+1, 4)] (dMean | dV | 0) and ONE partial block headpart [2*act + 5 + 2*hidden] =
  * db3p | db3c | dlogstd | pg vl kl cf sums | db2p | db2c.  scratch: >= m * (2*act + 8) + (m / 256 + 2) * max(2*hidden, 8) floats. */

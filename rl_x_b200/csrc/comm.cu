@@ -30,8 +30,7 @@ struct CommView {
 // one partial pair per CTA, so that no separate pass over the gradient is needed before clip + Adam.
 struct CommSumsq {
   float* partials;          // [gridDim.x, 2] or null
-  long long seg_off[RLX_PPO_NSEG + 1];
-  unsigned critic_mask;
+  PpoNetMap net;
   long long total;          // elements beyond `total` (the metric tail riding along) are not part of any norm
   long long* step_count;    // optional: incremented once (Adam's step counter, as ppo_grad_sumsq_kernel does)
 };
@@ -55,8 +54,6 @@ __device__ __forceinline__ unsigned long long global_ns() {
 // Peer data is read with ld.cv: peer lines must not be served from this SM's L1.
 // WORLD > 0: compile-time rank count, so that the peer loads of one element are all in flight before the first add (one NVLink round
 // trip per element instead of one per rank); WORLD == 0: any rank count.
-__device__ __forceinline__ int comm_net_of(const CommSumsq& q, long long i);
-
 template <int WORLD>
 __global__ void __launch_bounds__(kThreads) comm_allreduce_kernel(CommView v, int rank, int world_rt, unsigned long long seq,
                                                                    float* __restrict__ out, long long n, CommSumsq q) {
@@ -94,7 +91,7 @@ __global__ void __launch_bounds__(kThreads) comm_allreduce_kernel(CommView v, in
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           const long long idx = 4 * i + j;
-          if (idx < q.total) { if (comm_net_of(q, idx)) sc = fmaf(e[j], e[j], sc); else sp = fmaf(e[j], e[j], sp); }
+          if (idx < q.total) { if (net_of(q.net, idx)) sc = fmaf(e[j], e[j], sc); else sp = fmaf(e[j], e[j], sp); }
         }
       }
     } else {
@@ -111,7 +108,7 @@ __global__ void __launch_bounds__(kThreads) comm_allreduce_kernel(CommView v, in
       float acc = __ldcv(v.slot[0] + i);
       for (int r = 1; r < world; ++r) acc += __ldcv(v.slot[r] + i);
       out[i] = acc;
-      if (q.partials != nullptr && WORLD > 0 && i < q.total) { if (comm_net_of(q, i)) sc = fmaf(acc, acc, sc); else sp = fmaf(acc, acc, sp); }
+      if (q.partials != nullptr && WORLD > 0 && i < q.total) { if (net_of(q.net, i)) sc = fmaf(acc, acc, sc); else sp = fmaf(acc, acc, sp); }
     }
   }
   if (q.partials != nullptr && WORLD > 0) {
@@ -125,12 +122,6 @@ __global__ void __launch_bounds__(kThreads) comm_allreduce_kernel(CommView v, in
   }
 }
 
-__device__ __forceinline__ int comm_net_of(const CommSumsq& q, long long i) {
-  int seg = 0;
-#pragma unroll
-  for (int s = 1; s < RLX_PPO_NSEG; ++s) seg += (i >= q.seg_off[s]) ? 1 : 0;
-  return (q.critic_mask >> seg) & 1u;
-}
 __device__ __forceinline__ void wait_flag(const unsigned long long* f, unsigned long long seq, int rank, int peer, const char* what) {
   const unsigned long long t0 = global_ns();
   while (ld_acquire_sys(f) < seq) {
@@ -204,7 +195,7 @@ __global__ void __launch_bounds__(kThreads) comm_allreduce2_kernel(CommView v, i
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const long long idx = 4 * i + j;
-        if (idx < q.total) { if (comm_net_of(q, idx)) sc = fmaf(e[j], e[j], sc); else sp = fmaf(e[j], e[j], sp); }
+        if (idx < q.total) { if (net_of(q.net, idx)) sc = fmaf(e[j], e[j], sc); else sp = fmaf(e[j], e[j], sp); }
       }
     }
   }
@@ -212,7 +203,7 @@ __global__ void __launch_bounds__(kThreads) comm_allreduce2_kernel(CommView v, i
     for (long long i = (n4 << 2) + threadIdx.x; i < n; i += blockDim.x) {
       const float a = __ldcv(res + i);
       out[i] = a;
-      if (q.partials != nullptr && i < q.total) { if (comm_net_of(q, i)) sc = fmaf(a, a, sc); else sp = fmaf(a, a, sp); }
+      if (q.partials != nullptr && i < q.total) { if (net_of(q.net, i)) sc = fmaf(a, a, sc); else sp = fmaf(a, a, sp); }
     }
   }
   if (q.partials != nullptr) {
@@ -311,9 +302,7 @@ int comm_allreduce_ppo(rlx_comm* c, float* out, int64_t n, const rlx_ppo_dims& d
                        int* nblk_out) {
   CommSumsq q{};
   const PpoLayout L = make_layout(d);
-  for (int i = 0; i <= RLX_PPO_NSEG; ++i) q.seg_off[i] = L.off[i];
-  for (int i = 0; i < RLX_PPO_NSEG; ++i)
-    if (seg_is_critic(i)) q.critic_mask |= (1u << i);
+  q.net = make_net_map(L);
   q.total = L.total();
   q.partials = norm_partials;
   q.step_count = step_count;

@@ -142,6 +142,26 @@ inline PpoLayout make_layout(const rlx_ppo_dims& d) {
 }
 inline bool seg_is_critic(int s) { return s == W1C || s == B1C || s == W2C || s == B2C || s == W3C || s == B3C; }
 
+// Which net owns flat element i, in a form kernels can take by value (embedded in the parameter blocks of the norm kernels).
+struct PpoNetMap {
+  long long seg_off[RLX_PPO_NSEG + 1];
+  unsigned critic_mask;  // bit s set => segment s belongs to the critic
+};
+inline PpoNetMap make_net_map(const PpoLayout& L) {
+  PpoNetMap map{};
+  for (int i = 0; i <= RLX_PPO_NSEG; ++i) map.seg_off[i] = L.off[i];
+  for (int i = 0; i < RLX_PPO_NSEG; ++i)
+    if (seg_is_critic(i)) map.critic_mask |= (1u << i);
+  return map;
+}
+// 0 = policy, 1 = critic
+__device__ __forceinline__ int net_of(const PpoNetMap& map, long long i) {
+  int seg = 0;
+#pragma unroll
+  for (int s = 1; s < RLX_PPO_NSEG; ++s) seg += (i >= map.seg_off[s]) ? 1 : 0;
+  return (map.critic_mask >> seg) & 1u;
+}
+
 inline bool dims_ok(const rlx_ppo_dims& d) {
   return d.obs_dim > 0 && d.act_dim > 0 && d.hidden > 0 && d.act_dim <= 64 && d.hidden <= 4096 && d.obs_dim <= 65536;
 }

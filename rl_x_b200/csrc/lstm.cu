@@ -504,17 +504,6 @@ static int dense_fwd(const float* X, int ldx, const float* W, int in, int out, c
   g.splits = 1; g.kchunk = (int)(ceil_div(in, 8) * 8);
   return aux_gemm<true, false, EPI>(g, 1, st, KC_GEMM_FWD, R, in);
 }
-// backward wrt the input: C[r, i] = (sum_o dY[r, o] W[i, o]) [* (1 - aux[r, i]^2)]
-template <int EPI>
-static int dense_bwd_input(const float* dY, int ldy, const float* W, int in, int out, const float* aux, int ldaux, float* C, int ldc, long long R,
-                           cudaStream_t st) {
-  GemmP g{};
-  g.A = dY; g.B = W; g.C = C; g.aux = aux;
-  g.M = (int)R; g.N = in; g.K = out;
-  g.lda = ldy; g.ldb = out; g.ldc = ldc; g.ldaux = ldaux;
-  g.splits = 1; g.kchunk = (int)(ceil_div(out, 8) * 8);
-  return aux_gemm<true, true, EPI>(g, 1, st, KC_GEMM_DX, R, in);
-}
 // The same two products on a K-major copy WT [out, in] of the kernel (torch's Linear layout): these operand layouts are the ones every
 // epilogue of the tensor engine covers (bias, bias + tanh, tanh'), which the Flax layout [in, out] is not (gemm_tc.cu: RLX_TC_DISPATCH).
 template <int EPI>

@@ -70,6 +70,16 @@ static int launch_round_bf16(const float* src, float* dst, long long n, long lon
   RLX_LAUNCH_C(KC_OTHER, 0, 8.0 * n, round_bf16_kernel, grid, 256, 0, st, src, dst, n, keep_lo, keep_hi);
   return RLX_OK;
 }
+// bf16-autocast mode: points `params` and `X` (n_x floats) at rounded copies made in pr / xr (what autocast's casts hand to every Linear)
+static int round_inputs_bf16(const PpoLayout& L, const float*& params, const float*& X, long long n_x, float* pr, float* xr, cudaStream_t st) {
+  int rc = launch_round_bf16(params, pr, L.total(), L.off[LOGSTD], L.off[LOGSTD + 1], st);
+  if (rc) return rc;
+  rc = launch_round_bf16(X, xr, n_x, 0, 0, st);
+  if (rc) return rc;
+  params = pr;
+  X = xr;
+  return RLX_OK;
+}
 
 struct FwdPlan {
   size_t off_H1, off_H2, off_P, off_X, total;
@@ -104,8 +114,9 @@ static TrainPlan plan_train(const rlx_ppo_dims& d, long long m) {
   P.head_blocks = head_grid(m);
   P.head_npart = (int)(2 * A + 5 + 2 * H);
   P.wgrad_chunks = (int)ceil_div(m, kHeadWgradRows);
-  // one (policy, critic) partial pair per CTA of whichever kernel leaves the squared norms behind: the <= SM-count grids of the fused tail
-  // and of the exchange kernels, or the gradient-assembly grid (one CTA per 256 flat elements + one per 8 "tall" elements)
+  // one (policy, critic) partial pair per CTA of whichever kernel leaves the squared norms behind: the 64 CTAs of the sum-of-squares
+  // kernel, the <= SM-count grids of the exchange kernels, or the gradient-assembly grid (one CTA per 256 flat elements + one per 8 "tall"
+  // elements)
   P.norm_blocks = (int)std::max<long long>(std::max(64, sm_count()), ceil_div(make_layout(d).total(), 256) + ceil_div(2 * H + 2 * A + 1 + (A + 1) * H, 8) + 8);
   size_t o = 0;
   auto take = [&](size_t& off, size_t nfloats) {
@@ -194,9 +205,6 @@ static bool head_dims_ok(const rlx_ppo_dims& d) {
 
 int ppo_head_gemm_path(const HeadGemmArgs& a, cudaStream_t st);  // ppo_head_gemm.cu
 static int g_head_engine = 0;                                       // 0 fused SIMT kernel, 1 GEMM formulation, 2 fused mma.sync kernel (rlx_set_head_engine)
-// rlx_set_fused_tail(1): one-launch optimiser tail inside the epoch call.  Off by default: the <= SM-count grid that the grid barrier needs
-// leaves few threads in flight for the split-K partial reads (25 MB per minibatch), which the much larger grad_reduce grid hides.
-static int g_fused_tail = 0;
 
 static void fill_head_common(HeadP& h, const PpoLayout& L, const float* params, const float* H2, long long rows) {
   h.M = (int)rows; h.H = L.H; h.act = L.act;
@@ -237,14 +245,8 @@ extern "C" int rlx_ppo_forward_f32(const rlx_ppo_forward_args* a, void* stream) 
   const float* obs = a->obs;
   int rc;
   if (bf16) {
-    float* pr = ws_ptr<float>(a->workspace, P.off_P);
-    float* xr = ws_ptr<float>(a->workspace, P.off_X);
-    rc = launch_round_bf16(a->params, pr, L.total(), L.off[LOGSTD], L.off[LOGSTD + 1], st);
+    rc = round_inputs_bf16(L, params, obs, a->n * (long long)L.obs, ws_ptr<float>(a->workspace, P.off_P), ws_ptr<float>(a->workspace, P.off_X), st);
     if (rc) return rc;
-    rc = launch_round_bf16(a->obs, xr, a->n * (long long)L.obs, 0, 0, st);
-    if (rc) return rc;
-    params = pr;
-    obs = xr;
   }
   rc = mlp_hidden_forward(a->dims, L, params, obs, a->dims.obs_dim, a->n, H1, H2, st, bf16);
   if (rc) return rc;
@@ -276,7 +278,7 @@ extern "C" size_t rlx_ppo_minibatch_workspace_bytes(const rlx_ppo_dims* d, int64
   return plan_train(*d, std::max<int64_t>(m, 1)).total;
 }
 
-static int check_mb_args(const rlx_ppo_minibatch_args* a, bool need_data) {
+static int check_mb_args(const rlx_ppo_minibatch_args* a, bool need_data, TrainPlan& P) {
   RLX_CHECK_ARG(a != nullptr, "args is null");
   RLX_CHECK_ARG(head_dims_ok(a->dims), "unsupported dims (act <= 64, hidden <= 1024)");
   RLX_CHECK_ARG(a->m >= 0 && a->m < (1LL << 31) && a->m_global >= 1, "bad minibatch size");
@@ -284,7 +286,7 @@ static int check_mb_args(const rlx_ppo_minibatch_args* a, bool need_data) {
   if (need_data && a->m > 0) {
     RLX_CHECK_ARG(a->states && a->actions && a->log_probs && a->advantages && a->returns && a->adv_stats, "null minibatch tensor");
   }
-  const TrainPlan P = plan_train(a->dims, std::max<int64_t>(a->m, 1));
+  P = plan_train(a->dims, std::max<int64_t>(a->m, 1));
   if (a->workspace == nullptr || a->workspace_bytes < P.total) {
     set_error("rlx_ppo_minibatch: workspace too small (%zu < %zu)", a->workspace_bytes, P.total);
     return RLX_ERR_WORKSPACE;
@@ -310,96 +312,56 @@ static int launch_grad_reduce(const GradReduceP& r, cudaStream_t st) {
   return RLX_OK;
 }
 
-// `deferred`: when non-null the flat-gradient assembly is NOT launched; its parameters are returned for the fused optimiser tail.
-// `fuse_norms`: the assembly kernel also leaves the two squared clip norms in the workspace (off_barrier + 16 bytes) and bumps Adam's
-// step counter, so that clip + Adam can follow without the separate sum-of-squares launch.
-static int minibatch_fwdbwd(const rlx_ppo_minibatch_args* a, void* stream, GradReduceP* deferred, bool fuse_norms = false);
+// ---- stages of minibatch_fwdbwd, in launch order
+// the head kernels with the act <= 31 specialisations (and their dW3 kernels) cover the shape
+static bool fast_head_ok(const PpoLayout& L) { return (L.act <= 31) && (L.H % 2 == 0) && (L.H <= 1024); }
 
-extern "C" int rlx_ppo_minibatch_fwdbwd_f32(const rlx_ppo_minibatch_args* a, void* stream) { return minibatch_fwdbwd(a, stream, nullptr); }
-
-static int minibatch_fwdbwd(const rlx_ppo_minibatch_args* a, void* stream, GradReduceP* deferred, bool fuse_norms) {
-  int rc = check_mb_args(a, true);
-  if (rc) return rc;
-  const rlx_ppo_dims& d = a->dims;
-  const PpoLayout L = make_layout(d);
+// loss head: loss + dZ2 + dhead + block partials (incl. db2 = column sums of dZ2).  Returns the number of partial blocks written, < 0 on error.
+static int launch_train_head(const rlx_ppo_minibatch_args* a, const PpoLayout& L, const TrainPlan& P, const float* params, int bf16, cudaStream_t st) {
   const long long m = a->m;
-  const int H = L.H, O = L.obs, A = L.act;
-  const long long ldx = a->states_ld > 0 ? a->states_ld : O;
-  RLX_CHECK_ARG(ldx >= O, "states_ld smaller than obs_dim");
-  RLX_CHECK_ARG(!a->states_ones_col || ldx > O, "states_ones_col needs states_ld > obs_dim");
-  const bool tc = use_tc(d);
-  const TrainPlan P = plan_train(d, std::max<long long>(m, 1));
-  cudaStream_t st = (cudaStream_t)stream;
+  const int H = L.H, A = L.act;
   void* ws = a->workspace;
-  float* H1 = ws_ptr<float>(ws, P.off_H1);
   float* H2 = ws_ptr<float>(ws, P.off_H2);
   float* dZ2 = ws_ptr<float>(ws, P.off_dZ2);
-  float* dZ1 = ws_ptr<float>(ws, P.off_dZ1);
   float* dhead = ws_ptr<float>(ws, P.off_dhead);
   float* headpart = ws_ptr<float>(ws, P.off_headpart);
-  float* part1 = ws_ptr<float>(ws, P.off_part1);
-  float* rs1 = ws_ptr<float>(ws, P.off_rs1);
-  float* part2 = ws_ptr<float>(ws, P.off_part2);
-  float* part3 = ws_ptr<float>(ws, P.off_part3);
   const float inv_mg = 1.f / (float)a->m_global;
-  const int npart = P.head_npart;
-
-  int head_blocks = 0, wgrad_chunks = 0, s1 = 0, s2 = 0, w3_nsplit = 0;
-  long long w3_stride = (long long)(A + 1) * H, w3c_off = (long long)A * H;
-  const int bf16 = g_autocast_bf16;
-  const float* params = a->params;   // bf16 mode: the rounded copies below (what autocast's casts hand to every Linear)
-  const float* states = a->states;
-  if (m > 0) {
-    if (bf16) {
-      RLX_CHECK_ARG(ldx <= (long long)(ceil_div(O + 1, 4) * 4), "bf16 mode: states_ld larger than the planned rounded copy");
-      float* pr = ws_ptr<float>(ws, P.off_P);
-      float* xr = ws_ptr<float>(ws, P.off_X);
-      rc = launch_round_bf16(a->params, pr, L.total(), L.off[LOGSTD], L.off[LOGSTD + 1], st);
-      if (rc) return rc;
-      rc = launch_round_bf16(a->states, xr, m * ldx, 0, 0, st);
-      if (rc) return rc;
-      params = pr;
-      states = xr;
-    }
-    // ---- forward hidden layers
-    rc = mlp_hidden_forward(d, L, params, states, ldx, m, H1, H2, st, bf16);
+  HeadP h{};
+  fill_head_common(h, L, params, H2, m);
+  h.bf16 = bf16;
+  h.actions = a->actions; h.logp_old = a->log_probs; h.adv = a->advantages; h.ret = a->returns; h.adv_stats = a->adv_stats;
+  h.inv_mg = inv_mg; h.clip_range = a->hp.clip_range; h.critic_coef = a->hp.critic_coef;
+  h.ratio_delta_metric = a->hp.ratio_delta_metric != 0.f ? 1 : 0;
+  const bool want_median = a->hp.ratio_delta_metric == 2.f;  // ESPO delta_calc_operator = median (espo.py:59-60)
+  h.ratio_abs = want_median ? ws_ptr<float>(ws, P.off_ratio) : nullptr;
+  h.dZ2 = dZ2; h.dhead = dhead; h.block_partials = headpart;
+  int head_blocks = P.head_blocks;
+  const size_t smem = head_smem_bytes(a->dims, true);
+  const int dh_ld = (int)(ceil_div(A + 1, 4) * 4);
+  const bool fast_head = fast_head_ok(L);
+  const double head_flops = 4.0 * m * H * (A + 1), head_bytes = 4.0 * m * (4.0 * H + 2.0 * A + 5);
+  // opt-in GEMM formulation of the head (ppo_head_gemm.cu); dZ1 is free until the dX GEMM and serves as its scratch
+  const bool gemm_head = fast_head && g_head_engine == 1 && !bf16 && head_gemm_scratch_floats(m, H, A) <= m * 2LL * H;
+  if (gemm_head) {
+    HeadGemmArgs ha{m, H, A, dh_ld, H2, a->params + L.off[W3P], a->params + L.off[W3C], a->params + L.off[B3P], a->params + L.off[B3C],
+                    a->params + L.off[LOGSTD], a->actions, a->log_probs, a->advantages, a->returns, a->adv_stats, inv_mg, a->hp.clip_range,
+                    a->hp.critic_coef, a->hp.ratio_delta_metric != 0.f ? 1 : 0, dZ2, dhead, headpart, ws_ptr<float>(ws, P.off_dZ1)};
+    const int rc = ppo_head_gemm_path(ha, st);
     if (rc) return rc;
-    // ---- head: loss + dZ2 + dhead + block partials (incl. db2 = column sums of dZ2)
-    HeadP h{};
-    fill_head_common(h, L, params, H2, m);
-    h.bf16 = bf16;
-    h.actions = a->actions; h.logp_old = a->log_probs; h.adv = a->advantages; h.ret = a->returns; h.adv_stats = a->adv_stats;
-    h.inv_mg = inv_mg; h.clip_range = a->hp.clip_range; h.critic_coef = a->hp.critic_coef;
-    h.ratio_delta_metric = a->hp.ratio_delta_metric != 0.f ? 1 : 0;
-    const bool want_median = a->hp.ratio_delta_metric == 2.f;  // ESPO delta_calc_operator = median (espo.py:59-60)
-    h.ratio_abs = want_median ? ws_ptr<float>(ws, P.off_ratio) : nullptr;
-    h.dZ2 = dZ2; h.dhead = dhead; h.block_partials = headpart;
-    head_blocks = P.head_blocks;
-    const size_t smem = head_smem_bytes(d, true);
-    const int dh_ld = (int)(ceil_div(A + 1, 4) * 4);
-    const bool fast_head = (A <= 31) && (H % 2 == 0) && (H <= 1024);
-    const double head_flops = 4.0 * m * H * (A + 1), head_bytes = 4.0 * m * (4.0 * H + 2.0 * A + 5);
-    // opt-in GEMM formulation of the head (ppo_head_gemm.cu); dZ1 is free until the dX GEMM and serves as its scratch
-    const bool gemm_head = fast_head && g_head_engine == 1 && !bf16 && head_gemm_scratch_floats(m, H, A) <= m * 2LL * H;
-    if (gemm_head) {
-      HeadGemmArgs ha{m, H, A, dh_ld, H2, a->params + L.off[W3P], a->params + L.off[W3C], a->params + L.off[B3P], a->params + L.off[B3C],
-                      a->params + L.off[LOGSTD], a->actions, a->log_probs, a->advantages, a->returns, a->adv_stats, inv_mg, a->hp.clip_range,
-                      a->hp.critic_coef, a->hp.ratio_delta_metric != 0.f ? 1 : 0, dZ2, dhead, headpart, dZ1};
-      rc = ppo_head_gemm_path(ha, st);
-      if (rc) return rc;
-      head_blocks = 1;  // the path writes ONE partial block in the fused kernel's layout
-    }
-    if (fast_head) {
-      HeadTrain2Extra ex{dh_ld};
-      const bool vec_head = (H == 128 || H == 256 || H == 512);
-      // fused head on the warp-level tensor path (ppo_head_mma.cuh): fp32 mode, <= 4 n-tiles of 8 head columns
-      const int nt4 = (int)ceil_div(dh_ld, 8);
-      const size_t smem4 = head4_smem_floats(H, A, nt4) * sizeof(float);
-      const bool mma_head = !gemm_head && vec_head && g_head_engine == 2 && !bf16 && nt4 <= 4 && smem4 <= 220 * 1024;
-      if (gemm_head) {
-        // loss, dZ2, dhead and the partial block are done
-      } else if (mma_head) {
-        head_blocks = (int)std::min<long long>(ceil_div(m, 16 * kHead4RowTiles), (long long)P.head_blocks);
+    return 1;  // the path writes ONE partial block in the fused kernel's layout
+  }
+  if (!fast_head) {
+    RLX_DISPATCH_NCH(KC_HEAD_TRAIN, head_flops, head_bytes, H, ppo_head_train_kernel, head_blocks, 256, smem, st, h);
+    return head_blocks;
+  }
+  HeadTrain2Extra ex{dh_ld};
+  const bool vec_head = (H == 128 || H == 256 || H == 512);
+  // fused head on the warp-level tensor path (ppo_head_mma.cuh): fp32 mode, <= 4 n-tiles of 8 head columns
+  const int nt4 = (int)ceil_div(dh_ld, 8);
+  const size_t smem4 = head4_smem_floats(H, A, nt4) * sizeof(float);
+  const bool mma_head = vec_head && g_head_engine == 2 && !bf16 && nt4 <= 4 && smem4 <= 220 * 1024;
+  if (mma_head) {
+    head_blocks = (int)std::min<long long>(ceil_div(m, 16 * kHead4RowTiles), (long long)P.head_blocks);
 #define RLX_HEAD4(H_, NT_)                                                                                                          \
   do {                                                                                                                              \
     RLX_CHECK_CUDA(cudaFuncSetAttribute(ppo_head_train4_kernel<H_, NT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem4)); \
@@ -412,12 +374,12 @@ static int minibatch_fwdbwd(const rlx_ppo_minibatch_args* a, void* stream, GradR
     else if (nt4 == 3) RLX_HEAD4(H_, 3); \
     else RLX_HEAD4(H_, 4);            \
   } while (0)
-        if (H == 128) RLX_HEAD4_NT(128);
-        else if (H == 256) RLX_HEAD4_NT(256);
-        else RLX_HEAD4_NT(512);
+    if (H == 128) RLX_HEAD4_NT(128);
+    else if (H == 256) RLX_HEAD4_NT(256);
+    else RLX_HEAD4_NT(512);
 #undef RLX_HEAD4_NT
 #undef RLX_HEAD4
-      } else if (vec_head) {
+  } else if (vec_head) {
 #define RLX_HEAD3_B(H_, AM_, BF_)                                                                                                     \
   do {                                                                                                                                \
     RLX_CHECK_CUDA(cudaFuncSetAttribute(ppo_head_train3_kernel<H_, AM_, BF_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
@@ -435,14 +397,14 @@ static int minibatch_fwdbwd(const rlx_ppo_minibatch_args* a, void* stream, GradR
     else if (A <= 24) RLX_HEAD3(H_, 24);       \
     else RLX_HEAD3(H_, 31);                    \
   } while (0)
-        if (H == 128) RLX_HEAD3_ACT(128);
-        else if (H == 256) RLX_HEAD3_ACT(256);
-        else RLX_HEAD3_ACT(512);
+    if (H == 128) RLX_HEAD3_ACT(128);
+    else if (H == 256) RLX_HEAD3_ACT(256);
+    else RLX_HEAD3_ACT(512);
 #undef RLX_HEAD3_ACT
 #undef RLX_HEAD3
 #undef RLX_HEAD3_B
-      } else {
-        const int nch = (int)ceil_div(H, 32);
+  } else {
+    const int nch = (int)ceil_div(H, 32);
 #define RLX_HEAD2_B(NCH_, AM_, BF_)                                                                                                   \
   do {                                                                                                                                \
     RLX_CHECK_CUDA(cudaFuncSetAttribute(ppo_head_train2_kernel<NCH_, AM_, BF_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
@@ -460,158 +422,217 @@ static int minibatch_fwdbwd(const rlx_ppo_minibatch_args* a, void* stream, GradR
     else if (A <= 24) RLX_HEAD2(NCH_, 24);          \
     else RLX_HEAD2(NCH_, 31);                       \
   } while (0)
-        if (nch <= 2) RLX_HEAD2_ACT(2);
-        else if (nch <= 4) RLX_HEAD2_ACT(4);
-        else if (nch <= 8) RLX_HEAD2_ACT(8);
-        else if (nch <= 16) RLX_HEAD2_ACT(16);
-        else RLX_HEAD2_ACT(32);
+    if (nch <= 2) RLX_HEAD2_ACT(2);
+    else if (nch <= 4) RLX_HEAD2_ACT(4);
+    else if (nch <= 8) RLX_HEAD2_ACT(8);
+    else if (nch <= 16) RLX_HEAD2_ACT(16);
+    else RLX_HEAD2_ACT(32);
 #undef RLX_HEAD2_ACT
 #undef RLX_HEAD2
 #undef RLX_HEAD2_B
-      }
-      // ---- dW3 = dhead^T [act+1, m] . H2 [m, 2H]
-      bool w3_done = false;
-      if (tc) {
-        // tensor cores: one MN-major GEMM per net half (batch 2); the act+1 (padded to dh_ld) gradient columns are the M side
-        const Splits S3 = choose_splits(m, dh_ld, H, 2, true);
-        GemmP g3{};
-        g3.A = dhead; g3.B = H2; g3.C = part3;
-        g3.M = dh_ld; g3.N = H; g3.K = (int)m;
-        g3.lda = dh_ld; g3.ldb = 2 * H; g3.ldc = H;
-        g3.sA = 0; g3.sB = H; g3.sC = (long long)dh_ld * H;
-        g3.splits = S3.splits; g3.kchunk = S3.kchunk; g3.sSplitC = 2LL * dh_ld * H;
-        g3.bf16 = bf16;
-        rc = tc_gemm(g3, false, false, TC_NONE, 2, KC_HEAD_WGRAD, m, m, 0, nullptr, 0, 0, st);
-        if (rc == RLX_OK) {
-          w3_done = true;
-          w3_nsplit = S3.splits;
-          w3_stride = 2LL * dh_ld * H;
-          w3c_off = (long long)dh_ld * H + (long long)A * H;  // net 1 (critic half of H2), row `act` of its [dh_ld, H] block
-        } else if (rc != RLX_ERR_UNSUPPORTED) {
-          return rc;
-        }
-      }
-      if (!w3_done) {
-        // SIMT: one thread per (policy, critic) column pair, 64 rows per CTA
-        HeadWgrad2P w{(int)m, H, A, dh_ld, kHeadWgradRows, H2, dhead, part3};
-        wgrad_chunks = (int)ceil_div(m, kHeadWgradRows);
-        const unsigned wthreads = (unsigned)(ceil_div(H, 32) * 32);
-        const size_t wsmem = (size_t)kHeadWgradRows * dh_ld * sizeof(float);
-        const double wflops = 2.0 * m * H * (A + 1), wbytes = 4.0 * m * (2.0 * H + A + 1);
-        if (A + 1 <= 4) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<4>, wgrad_chunks, wthreads, wsmem, st, w);
-        else if (A + 1 <= 8) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<8>, wgrad_chunks, wthreads, wsmem, st, w);
-        else if (A + 1 <= 12) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<12>, wgrad_chunks, wthreads, wsmem, st, w);
-        else if (A + 1 <= 16) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<16>, wgrad_chunks, wthreads, wsmem, st, w);
-        else if (A + 1 <= 20) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<20>, wgrad_chunks, wthreads, wsmem, st, w);
-        else if (A + 1 <= 24) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<24>, wgrad_chunks, wthreads, wsmem, st, w);
-        else RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<32>, wgrad_chunks, wthreads, wsmem, st, w);
-        w3_nsplit = wgrad_chunks;
-      }
-    } else {
-      RLX_DISPATCH_NCH(KC_HEAD_TRAIN, head_flops, head_bytes, H, ppo_head_train_kernel, head_blocks, 256, smem, st, h);
-      // ---- dW3 (thread per column, chunked over rows)
-      HeadWgradP w{(int)m, H, A, kHeadWgradRows, H2, dhead, part3};
-      wgrad_chunks = (int)ceil_div(m, kHeadWgradRows);
-      dim3 wg((unsigned)wgrad_chunks, (unsigned)ceil_div(2 * H, 256));
-      const size_t wsmem = (size_t)kHeadWgradRows * (A + 1) * sizeof(float);
-      if (A <= 8) {
-        RLX_LAUNCH_C(KC_HEAD_WGRAD, 2.0 * m * H * (A + 1), 4.0 * m * (2.0 * H + A + 1), ppo_head_wgrad_kernel<8>, wg, 256, wsmem, st, w);
-      } else if (A <= 32) {
-        RLX_LAUNCH_C(KC_HEAD_WGRAD, 2.0 * m * H * (A + 1), 4.0 * m * (2.0 * H + A + 1), ppo_head_wgrad_kernel<32>, wg, 256, wsmem, st, w);
-      } else {
-        RLX_CHECK_CUDA(cudaFuncSetAttribute(ppo_head_wgrad_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem));
-        RLX_LAUNCH_C(KC_HEAD_WGRAD, 2.0 * m * H * (A + 1), 4.0 * m * (2.0 * H + A + 1), ppo_head_wgrad_kernel<64>, wg, 256, wsmem, st, w);
-      }
-      w3_nsplit = wgrad_chunks;
-    }
-    // ---- dW2 : part2[split][net][o][i] = sum_rows dZ2[r, net*H+o] * H1[r, net*H+i]   (db2 comes from the head kernel)
-    const Splits S2 = choose_splits(m, H, H, 2, tc);
-    s2 = S2.splits;
-    GemmP g{};
-    g.A = dZ2; g.B = H1; g.C = part2;
-    g.M = H; g.N = H; g.K = (int)m;
-    g.lda = 2 * H; g.ldb = 2 * H; g.ldc = H;
-    g.sA = H; g.sB = H; g.sC = (long long)H * H;
-    g.splits = S2.splits; g.kchunk = S2.kchunk; g.sSplitC = 2LL * H * H;
-    g.bf16 = bf16;
-    rc = run_gemm<false, false, EPI_NONE>(tc, g, 2, st, KC_GEMM_DW, m, m);
-    if (rc) return rc;
-    // ---- dZ1 = (dZ2 @ W2) * (1 - H1^2)   per net
-    GemmP gd{};
-    gd.A = dZ2; gd.B = params + L.off[W2P]; gd.C = dZ1; gd.aux = H1;
-    gd.bf16 = bf16;
-    gd.M = (int)m; gd.N = H; gd.K = H;
-    gd.lda = 2 * H; gd.ldb = H; gd.ldc = 2 * H; gd.ldaux = 2 * H;
-    gd.sA = H; gd.sB = (long long)H * H; gd.sC = H; gd.sAux = H;
-    gd.splits = 1; gd.kchunk = (int)(ceil_div(H, 8) * 8);
-    rc = run_gemm<true, false, EPI_DTANH>(tc, gd, 2, st, KC_GEMM_DX, m, H);
-    if (rc) return rc;
-    // ---- dW1cat | db1cat : part1[split][o][i] = sum_rows dZ1[r, o] * X[r, i];  db1[o] = sum_rows dZ1[r, o]
-    GemmP g1{};
-    g1.A = dZ1; g1.B = states; g1.C = part1;
-    g1.bf16 = bf16;
-    g1.M = 2 * H; g1.N = O; g1.K = (int)m;
-    g1.lda = 2 * H; g1.ldb = (int)ldx; g1.ldc = O;
-    bool done = false;
-    if (tc && a->states_ones_col) {
-      // tensor-core path, computed TRANSPOSED: C^T[i, o] = sum_r X_aug[r, i] dZ1[r, o] with M = O+1 (the constant-one column of X
-      // makes db1 the last output row) and N = 2H = whole 128-wide tiles; the epilogue stores C^T transposed back into [o][i].
-      const Splits S1 = choose_splits(m, O + 1, 2 * H, 1, true);
-      GemmP gt{};
-      gt.A = states; gt.B = dZ1; gt.C = part1;
-      gt.bf16 = bf16;
-      gt.M = O + 1; gt.N = 2 * H; gt.K = (int)m;
-      gt.lda = (int)ldx; gt.ldb = 2 * H; gt.ldc = O;
-      gt.splits = S1.splits; gt.kchunk = S1.kchunk; gt.sSplitC = 2LL * H * O;
-      rc = tc_gemm_t(gt, false, false, TC_NONE, 1, KC_GEMM_DW, m, m, 0, rs1, 0, 2LL * H, st, 1, O);
-      if (rc == RLX_OK) {
-        done = true;
-        s1 = S1.splits;
-      } else if (rc != RLX_ERR_UNSUPPORTED) {
-        return rc;
-      }
-    }
-    if (!done) {
-      const Splits S1 = choose_splits(m, 2 * H, O, 1, false);
-      s1 = S1.splits;
-      g1.rowsum = rs1;
-      g1.splits = S1.splits; g1.kchunk = S1.kchunk; g1.sSplitC = 2LL * H * O; g1.sSplitRowsum = 2LL * H;
-      rc = launch_sgemm<false, false, EPI_NONE>(g1, 1, st, KC_GEMM_DW);
-      if (rc) return rc;
-    }
   }
-  // ---- assemble the flat gradient (m == 0: a rank that owns no row of this minibatch contributes zeros)
+  return head_blocks;
+}
+
+// Where the dW3 partials are: split s of dW3p [act, H] at src + s * stride, of dW3c [H] at src + critic_off + s * stride.
+struct W3Partials {
+  float* src;
+  int nsplit;
+  long long stride, critic_off;
+};
+// the layout of the SIMT kernels: part[chunk][(act+1)*H], rows 0..act-1 = dW3p, row act = dW3c
+static W3Partials chunked_w3(const PpoLayout& L, float* part3, int nchunks) {
+  return W3Partials{part3, nchunks, (long long)(L.act + 1) * L.H, (long long)L.act * L.H};
+}
+
+// dW3 = dhead^T [act+1, m] . H2 [m, 2H]
+static int launch_head_wgrad(const PpoLayout& L, const TrainPlan& P, long long m, bool tc, int bf16, void* ws, cudaStream_t st, W3Partials& w3) {
+  const int H = L.H, A = L.act;
+  float* H2 = ws_ptr<float>(ws, P.off_H2);
+  float* dhead = ws_ptr<float>(ws, P.off_dhead);
+  float* part3 = ws_ptr<float>(ws, P.off_part3);
+  const int wgrad_chunks = (int)ceil_div(m, kHeadWgradRows);
+  const double wflops = 2.0 * m * H * (A + 1), wbytes = 4.0 * m * (2.0 * H + A + 1);
+  if (!fast_head_ok(L)) {
+    // thread per column, chunked over rows
+    HeadWgradP w{(int)m, H, A, kHeadWgradRows, H2, dhead, part3};
+    dim3 wg((unsigned)wgrad_chunks, (unsigned)ceil_div(2 * H, 256));
+    const size_t wsmem = (size_t)kHeadWgradRows * (A + 1) * sizeof(float);
+    if (A <= 8) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad_kernel<8>, wg, 256, wsmem, st, w);
+    else if (A <= 32) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad_kernel<32>, wg, 256, wsmem, st, w);
+    else {
+      RLX_CHECK_CUDA(cudaFuncSetAttribute(ppo_head_wgrad_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem));
+      RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad_kernel<64>, wg, 256, wsmem, st, w);
+    }
+    w3 = chunked_w3(L, part3, wgrad_chunks);
+    return RLX_OK;
+  }
+  const int dh_ld = (int)(ceil_div(A + 1, 4) * 4);
+  if (tc) {
+    // tensor cores: one MN-major GEMM per net half (batch 2); the act+1 (padded to dh_ld) gradient columns are the M side
+    const Splits S3 = choose_splits(m, dh_ld, H, 2, true);
+    GemmP g3{};
+    g3.A = dhead; g3.B = H2; g3.C = part3;
+    g3.M = dh_ld; g3.N = H; g3.K = (int)m;
+    g3.lda = dh_ld; g3.ldb = 2 * H; g3.ldc = H;
+    g3.sA = 0; g3.sB = H; g3.sC = (long long)dh_ld * H;
+    g3.splits = S3.splits; g3.kchunk = S3.kchunk; g3.sSplitC = 2LL * dh_ld * H;
+    g3.bf16 = bf16;
+    const int rc = tc_gemm(g3, false, false, TC_NONE, 2, KC_HEAD_WGRAD, m, m, 0, nullptr, 0, 0, st);
+    if (rc == RLX_OK) {
+      // net 1 (critic half of H2), row `act` of its [dh_ld, H] block
+      w3 = W3Partials{part3, S3.splits, 2LL * dh_ld * H, (long long)dh_ld * H + (long long)A * H};
+      return RLX_OK;
+    }
+    if (rc != RLX_ERR_UNSUPPORTED) return rc;
+  }
+  // SIMT: one thread per (policy, critic) column pair, 64 rows per CTA
+  HeadWgrad2P w{(int)m, H, A, dh_ld, kHeadWgradRows, H2, dhead, part3};
+  const unsigned wthreads = (unsigned)(ceil_div(H, 32) * 32);
+  const size_t wsmem = (size_t)kHeadWgradRows * dh_ld * sizeof(float);
+  if (A + 1 <= 4) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<4>, wgrad_chunks, wthreads, wsmem, st, w);
+  else if (A + 1 <= 8) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<8>, wgrad_chunks, wthreads, wsmem, st, w);
+  else if (A + 1 <= 12) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<12>, wgrad_chunks, wthreads, wsmem, st, w);
+  else if (A + 1 <= 16) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<16>, wgrad_chunks, wthreads, wsmem, st, w);
+  else if (A + 1 <= 20) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<20>, wgrad_chunks, wthreads, wsmem, st, w);
+  else if (A + 1 <= 24) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<24>, wgrad_chunks, wthreads, wsmem, st, w);
+  else RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<32>, wgrad_chunks, wthreads, wsmem, st, w);
+  w3 = chunked_w3(L, part3, wgrad_chunks);
+  return RLX_OK;
+}
+
+// hidden layers backward: dW2, dZ1, dW1 | db1 (split over rows; s1 / s2 = split counts of the dW1 | db1 / dW2 partials)
+static int launch_hidden_backward(const PpoLayout& L, const TrainPlan& P, const float* params, const float* states, long long ldx, bool ones_col,
+                                  long long m, bool tc, int bf16, void* ws, cudaStream_t st, int& s1, int& s2) {
+  const int H = L.H, O = L.obs;
+  float* H1 = ws_ptr<float>(ws, P.off_H1);
+  float* dZ2 = ws_ptr<float>(ws, P.off_dZ2);
+  float* dZ1 = ws_ptr<float>(ws, P.off_dZ1);
+  float* part1 = ws_ptr<float>(ws, P.off_part1);
+  float* rs1 = ws_ptr<float>(ws, P.off_rs1);
+  float* part2 = ws_ptr<float>(ws, P.off_part2);
+  // ---- dW2 : part2[split][net][o][i] = sum_rows dZ2[r, net*H+o] * H1[r, net*H+i]   (db2 comes from the head kernel)
+  const Splits S2 = choose_splits(m, H, H, 2, tc);
+  s2 = S2.splits;
+  GemmP g{};
+  g.A = dZ2; g.B = H1; g.C = part2;
+  g.M = H; g.N = H; g.K = (int)m;
+  g.lda = 2 * H; g.ldb = 2 * H; g.ldc = H;
+  g.sA = H; g.sB = H; g.sC = (long long)H * H;
+  g.splits = S2.splits; g.kchunk = S2.kchunk; g.sSplitC = 2LL * H * H;
+  g.bf16 = bf16;
+  int rc = run_gemm<false, false, EPI_NONE>(tc, g, 2, st, KC_GEMM_DW, m, m);
+  if (rc) return rc;
+  // ---- dZ1 = (dZ2 @ W2) * (1 - H1^2)   per net
+  GemmP gd{};
+  gd.A = dZ2; gd.B = params + L.off[W2P]; gd.C = dZ1; gd.aux = H1;
+  gd.bf16 = bf16;
+  gd.M = (int)m; gd.N = H; gd.K = H;
+  gd.lda = 2 * H; gd.ldb = H; gd.ldc = 2 * H; gd.ldaux = 2 * H;
+  gd.sA = H; gd.sB = (long long)H * H; gd.sC = H; gd.sAux = H;
+  gd.splits = 1; gd.kchunk = (int)(ceil_div(H, 8) * 8);
+  rc = run_gemm<true, false, EPI_DTANH>(tc, gd, 2, st, KC_GEMM_DX, m, H);
+  if (rc) return rc;
+  // ---- dW1cat | db1cat : part1[split][o][i] = sum_rows dZ1[r, o] * X[r, i];  db1[o] = sum_rows dZ1[r, o]
+  if (tc && ones_col) {
+    // tensor-core path, computed TRANSPOSED: C^T[i, o] = sum_r X_aug[r, i] dZ1[r, o] with M = O+1 (the constant-one column of X
+    // makes db1 the last output row) and N = 2H = whole 128-wide tiles; the epilogue stores C^T transposed back into [o][i].
+    const Splits S1 = choose_splits(m, O + 1, 2 * H, 1, true);
+    GemmP gt{};
+    gt.A = states; gt.B = dZ1; gt.C = part1;
+    gt.bf16 = bf16;
+    gt.M = O + 1; gt.N = 2 * H; gt.K = (int)m;
+    gt.lda = (int)ldx; gt.ldb = 2 * H; gt.ldc = O;
+    gt.splits = S1.splits; gt.kchunk = S1.kchunk; gt.sSplitC = 2LL * H * O;
+    rc = tc_gemm_t(gt, false, false, TC_NONE, 1, KC_GEMM_DW, m, m, 0, rs1, 0, 2LL * H, st, 1, O);
+    if (rc == RLX_OK) {
+      s1 = S1.splits;
+      return RLX_OK;
+    }
+    if (rc != RLX_ERR_UNSUPPORTED) return rc;
+  }
+  const Splits S1 = choose_splits(m, 2 * H, O, 1, false);
+  s1 = S1.splits;
+  GemmP g1{};
+  g1.A = dZ1; g1.B = states; g1.C = part1;
+  g1.bf16 = bf16;
+  g1.M = 2 * H; g1.N = O; g1.K = (int)m;
+  g1.lda = 2 * H; g1.ldb = (int)ldx; g1.ldc = O;
+  g1.rowsum = rs1;
+  g1.splits = S1.splits; g1.kchunk = S1.kchunk; g1.sSplitC = 2LL * H * O; g1.sSplitRowsum = 2LL * H;
+  return launch_sgemm<false, false, EPI_NONE>(g1, 1, st, KC_GEMM_DW);
+}
+
+// assembly of the flat gradient from the partials the stages left (m == 0: a rank that owns no row of this minibatch contributes zeros)
+static GradReduceP make_grad_reduce(const rlx_ppo_minibatch_args* a, const PpoLayout& L, const TrainPlan& P, int head_blocks, const W3Partials& w3,
+                                    int s1, int s2, bool fuse_norms) {
+  const int H = L.H, O = L.obs, A = L.act;
+  void* ws = a->workspace;
+  const float* headpart = ws_ptr<float>(ws, P.off_headpart);
+  const int npart = P.head_npart;
+  const float inv_mg = 1.f / (float)a->m_global;
   GradReduceP r{};
-  r.g[0] = GradGroup{L.off[W1P], 2LL * H * O, part1, s1, 2LL * H * O};
-  r.g[1] = GradGroup{L.off[B1P], 2LL * H, rs1, s1, 2LL * H};
-  r.g[2] = GradGroup{L.off[W2P], 2LL * H * H, part2, s2, 2LL * H * H};
+  r.g[0] = GradGroup{L.off[W1P], 2LL * H * O, ws_ptr<float>(ws, P.off_part1), s1, 2LL * H * O};
+  r.g[1] = GradGroup{L.off[B1P], 2LL * H, ws_ptr<float>(ws, P.off_rs1), s1, 2LL * H};
+  r.g[2] = GradGroup{L.off[W2P], 2LL * H * H, ws_ptr<float>(ws, P.off_part2), s2, 2LL * H * H};
   r.g[3] = GradGroup{L.off[B2P], 2LL * H, headpart + (2 * A + 5), head_blocks, (long long)npart};
-  r.g[4] = GradGroup{L.off[W3P], (long long)A * H, part3, w3_nsplit, w3_stride};
+  r.g[4] = GradGroup{L.off[W3P], (long long)A * H, w3.src, w3.nsplit, w3.stride};
   r.g[5] = GradGroup{L.off[B3P], 2LL * A + 1, headpart, head_blocks, (long long)npart};
-  r.g[6] = GradGroup{L.off[W3C], (long long)H, part3 + w3c_off, w3_nsplit, w3_stride};
+  r.g[6] = GradGroup{L.off[W3C], (long long)H, w3.src + w3.critic_off, w3.nsplit, w3.stride};
   r.total = L.total();
   r.logstd_off = L.off[LOGSTD];
   r.act = A;
-  r.entropy_grad = -a->hp.entropy_coef * (float)m * inv_mg;
+  r.entropy_grad = -a->hp.entropy_coef * (float)a->m * inv_mg;
   r.grads = a->grads;
   r.head_partials = headpart; r.nblk = head_blocks; r.npart = npart; r.inv_mg = inv_mg; r.critic_coef = a->hp.critic_coef;
   r.logstd = a->params + L.off[LOGSTD];
-  r.metrics = a->metrics; r.m_local = (float)m;
-  r.bf16 = bf16;
-  if (fuse_norms && deferred == nullptr) {
+  r.metrics = a->metrics; r.m_local = (float)a->m;
+  r.bf16 = g_autocast_bf16;
+  if (fuse_norms) {
     r.norm_partials = ws_ptr<float>(ws, P.off_norm);
     r.done = ws_ptr<unsigned int>(ws, P.off_barrier);
     r.norm_out = ws_ptr<float>(ws, P.off_barrier) + 4;
     r.step_count = (long long*)a->step_count;
-    for (int i = 0; i <= RLX_PPO_NSEG; ++i) r.seg_off[i] = L.off[i];
-    for (int i = 0; i < RLX_PPO_NSEG; ++i)
-      if (seg_is_critic(i)) r.critic_mask |= (1u << i);
+    r.net = make_net_map(L);
   }
-  if (deferred != nullptr) {
-    *deferred = r;
-    return RLX_OK;
+  return r;
+}
+
+// `fuse_norms`: the assembly kernel also leaves the two squared clip norms in the workspace (off_barrier + 16 bytes) and bumps Adam's
+// step counter, so that clip + Adam can follow without the separate sum-of-squares launch.
+static int minibatch_fwdbwd(const rlx_ppo_minibatch_args* a, void* stream, bool fuse_norms = false) {
+  TrainPlan P;
+  int rc = check_mb_args(a, true, P);
+  if (rc) return rc;
+  const PpoLayout L = make_layout(a->dims);
+  const long long m = a->m;
+  const long long ldx = a->states_ld > 0 ? a->states_ld : L.obs;
+  RLX_CHECK_ARG(ldx >= L.obs, "states_ld smaller than obs_dim");
+  RLX_CHECK_ARG(!a->states_ones_col || ldx > L.obs, "states_ones_col needs states_ld > obs_dim");
+  const bool tc = use_tc(a->dims);
+  const int bf16 = g_autocast_bf16;
+  cudaStream_t st = (cudaStream_t)stream;
+  void* ws = a->workspace;
+  int head_blocks = 0, s1 = 0, s2 = 0;
+  W3Partials w3 = chunked_w3(L, ws_ptr<float>(ws, P.off_part3), 0);
+  if (m > 0) {
+    const float* params = a->params;
+    const float* states = a->states;
+    if (bf16) {
+      RLX_CHECK_ARG(ldx <= (long long)(ceil_div(L.obs + 1, 4) * 4), "bf16 mode: states_ld larger than the planned rounded copy");
+      rc = round_inputs_bf16(L, params, states, m * ldx, ws_ptr<float>(ws, P.off_P), ws_ptr<float>(ws, P.off_X), st);
+      if (rc) return rc;
+    }
+    rc = mlp_hidden_forward(a->dims, L, params, states, ldx, m, ws_ptr<float>(ws, P.off_H1), ws_ptr<float>(ws, P.off_H2), st, bf16);
+    if (rc) return rc;
+    head_blocks = launch_train_head(a, L, P, params, bf16, st);
+    if (head_blocks < 0) return head_blocks;
+    rc = launch_head_wgrad(L, P, m, tc, bf16, ws, st, w3);
+    if (rc) return rc;
+    rc = launch_hidden_backward(L, P, params, states, ldx, a->states_ones_col, m, tc, bf16, ws, st, s1, s2);
+    if (rc) return rc;
   }
-  rc = launch_grad_reduce(r, st);
+  rc = launch_grad_reduce(make_grad_reduce(a, L, P, head_blocks, w3, s1, s2, fuse_norms), st);
   if (rc) return rc;
   if (a->hp.ratio_delta_metric == 2.f && m > 0 && a->metrics != nullptr) {
     // metrics[4] <- torch.median(|ratio - 1|) of this minibatch, overwriting the mean the assembly kernel has just put there
@@ -620,110 +641,86 @@ static int minibatch_fwdbwd(const rlx_ppo_minibatch_args* a, void* stream, GradR
   return RLX_OK;
 }
 
-static AdamP make_adam_params(const rlx_ppo_minibatch_args* a, const PpoLayout& L, const TrainPlan& P) {
+extern "C" int rlx_ppo_minibatch_fwdbwd_f32(const rlx_ppo_minibatch_args* a, void* stream) { return minibatch_fwdbwd(a, stream); }
+
+static AdamP make_adam_params(const rlx_ppo_minibatch_args* a, const PpoLayout& L, float* norm_partials, int nblk_norm) {
   AdamP p{};
   p.total = L.total();
-  for (int i = 0; i <= RLX_PPO_NSEG; ++i) p.seg_off[i] = L.off[i];
-  p.critic_mask = 0;
-  for (int i = 0; i < RLX_PPO_NSEG; ++i)
-    if (seg_is_critic(i)) p.critic_mask |= (1u << i);
+  p.net = make_net_map(L);
   p.params = a->params; p.grads = a->grads; p.m = a->exp_avg; p.v = a->exp_avg_sq;
   p.lr = a->lr; p.step_count = (long long*)a->step_count;
   p.max_norm = a->hp.max_grad_norm; p.beta1 = a->hp.adam_beta1; p.beta2 = a->hp.adam_beta2; p.eps = a->hp.adam_eps;
-  p.norm_partials = ws_ptr<float>(a->workspace, P.off_norm);
-  p.nblk_norm = P.norm_blocks;
+  p.norm_partials = norm_partials;
+  p.nblk_norm = nblk_norm;
   p.metrics = a->metrics;
   return p;
 }
 
-extern "C" int rlx_gradnorm_clip_adam_f32(const rlx_ppo_minibatch_args* a, void* stream) {
-  int rc = check_mb_args(a, false);
-  if (rc) return rc;
-  RLX_CHECK_ARG(a->exp_avg && a->exp_avg_sq && a->lr && a->step_count, "optimizer state is null");
-  const PpoLayout L = make_layout(a->dims);
-  const TrainPlan P = plan_train(a->dims, std::max<int64_t>(a->m, 1));
-  cudaStream_t st = (cudaStream_t)stream;
-  AdamP p = make_adam_params(a, L, P);
-  p.nblk_norm = 64;
-  RLX_LAUNCH_C(KC_CLIP_ADAM, 0, 4.0 * L.total(), ppo_grad_sumsq_kernel, (unsigned)p.nblk_norm, 256, 0, st, p);
+// clip + Adam, the two squared norms summed from `nblk` (policy, critic) partial pairs at `norm_partials`
+static int launch_clip_adam(const rlx_ppo_minibatch_args* a, const PpoLayout& L, float* norm_partials, int nblk, cudaStream_t st) {
+  const AdamP p = make_adam_params(a, L, norm_partials, nblk);
   RLX_LAUNCH_C(KC_CLIP_ADAM, 0, 28.0 * L.total(), ppo_clip_adam_kernel, (unsigned)ceil_div(L.total(), 256), 256, 0, st, p);
   return RLX_OK;
 }
 
+extern "C" int rlx_gradnorm_clip_adam_f32(const rlx_ppo_minibatch_args* a, void* stream) {
+  TrainPlan P;
+  int rc = check_mb_args(a, false, P);
+  if (rc) return rc;
+  RLX_CHECK_ARG(a->exp_avg && a->exp_avg_sq && a->lr && a->step_count, "optimizer state is null");
+  const PpoLayout L = make_layout(a->dims);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int nblk = 64;
+  float* partials = ws_ptr<float>(a->workspace, P.off_norm);
+  const AdamP p = make_adam_params(a, L, partials, nblk);
+  RLX_LAUNCH_C(KC_CLIP_ADAM, 0, 4.0 * L.total(), ppo_grad_sumsq_kernel, (unsigned)nblk, 256, 0, st, p);
+  return launch_clip_adam(a, L, partials, nblk, st);
+}
+
+// minibatch k of an epoch: m gathered rows from row r0 on, and row k of the advantage statistics
+static rlx_ppo_minibatch_args minibatch_slice(const rlx_ppo_minibatch_args* first, int64_t k, int64_t r0, int64_t m) {
+  const int64_t ld = first->states_ld > 0 ? first->states_ld : first->dims.obs_dim;  // row pitch of the gathered states
+  rlx_ppo_minibatch_args a = *first;
+  a.m = m;
+  a.states = first->states + r0 * ld;
+  a.actions = first->actions + r0 * first->dims.act_dim;
+  a.log_probs = first->log_probs + r0;
+  a.advantages = first->advantages + r0;
+  a.returns = first->returns + r0;
+  a.adv_stats = first->adv_stats + 2 * k;
+  return a;
+}
+
 extern "C" int rlx_ppo_update_epoch_f32(const rlx_ppo_minibatch_args* first, int64_t count, int64_t mb, void* stream) {
   RLX_CHECK_ARG(first != nullptr && count >= 0 && mb > 0, "bad arguments");
-  const int64_t nmb = ceil_div(count, mb);
-  const int A = first->dims.act_dim;
-  const int64_t O = first->states_ld > 0 ? first->states_ld : first->dims.obs_dim;  // row pitch of the gathered states
-  // fused optimiser tail (ppo_optim.cuh): every thread of a <= SM-count grid keeps its gradient elements in registers across a grid
-  // barrier.  Needs the whole flat gradient to fit (kTailPerThread elements per thread) and the tall groups (head bias partials: 2H +
-  // 2A + 1 elements, W3 when it comes from the SIMT head) to fit two per warp; otherwise the three separate kernels run.
+  const int64_t nmb = ceil_div(count, mb), full = std::min<int64_t>(mb, count);
   cudaStream_t st = (cudaStream_t)stream;
-  bool fused = g_fused_tail && dims_ok(first->dims) && first->exp_avg && first->exp_avg_sq && first->lr && first->step_count && first->workspace;
-  const PpoLayout L = fused ? make_layout(first->dims) : PpoLayout{};
-  unsigned tail_grid = 0;
   // clip norms fused into the gradient-assembly kernel (needs the optimiser state and the ticket word in the workspace zeroed once)
-  bool norms_in_reduce = !fused && dims_ok(first->dims) && first->exp_avg && first->exp_avg_sq && first->lr && first->step_count && first->workspace;
+  bool norms_in_reduce = dims_ok(first->dims) && first->exp_avg && first->exp_avg_sq && first->lr && first->step_count && first->workspace;
+  TrainPlan P{};
   if (norms_in_reduce) {
-    const TrainPlan P0 = plan_train(first->dims, std::max<int64_t>(std::min<int64_t>(mb, count), 1));
-    if (first->workspace_bytes < P0.total) norms_in_reduce = false;
-    else RLX_CHECK_CUDA(cudaMemsetAsync(ws_ptr<unsigned int>(first->workspace, P0.off_barrier), 0, 64, st));
-  }
-  if (fused) {
-    tail_grid = (unsigned)std::min<int64_t>(sm_count(), ceil_div(L.total(), kTailThreads));
-    fused = (int64_t)tail_grid * kTailThreads * kTailPerThread >= L.total();
-    if (fused) {
-      const TrainPlan P0 = plan_train(first->dims, std::max<int64_t>(std::min<int64_t>(mb, count), 1));
-      if (first->workspace_bytes < P0.total) fused = false;  // the per-minibatch checks below will report it
-      else RLX_CHECK_CUDA(cudaMemsetAsync(ws_ptr<unsigned int>(first->workspace, P0.off_barrier), 0, 64, st));
-    }
+    P = plan_train(first->dims, std::max<int64_t>(full, 1));
+    if (first->workspace_bytes < P.total) norms_in_reduce = false;
+    else RLX_CHECK_CUDA(cudaMemsetAsync(ws_ptr<unsigned int>(first->workspace, P.off_barrier), 0, 64, st));
   }
   for (int64_t k = 0; k < nmb; ++k) {
-    rlx_ppo_minibatch_args a = *first;
-    const int64_t r0 = k * mb;
-    a.m = std::min<int64_t>(mb, count - r0);
+    rlx_ppo_minibatch_args a = minibatch_slice(first, k, k * mb, std::min<int64_t>(mb, count - k * mb));
     a.m_global = a.m;
-    a.states = first->states + r0 * O;
-    a.actions = first->actions + r0 * A;
-    a.log_probs = first->log_probs + r0;
-    a.advantages = first->advantages + r0;
-    a.returns = first->returns + r0;
-    a.adv_stats = first->adv_stats + 2 * k;
     a.metrics = first->metrics ? first->metrics + RLX_PPO_NMETRIC * k : nullptr;
-    if (!fused && norms_in_reduce && a.m == std::min<int64_t>(mb, count)) {
-      // default: the assembly kernel leaves the clip norms behind; clip + Adam read them (no separate sum-of-squares launch)
-      int rc = minibatch_fwdbwd(&a, stream, nullptr, true);
+    int rc;
+    if (norms_in_reduce && a.m == full) {
+      // the assembly kernel leaves the clip norms behind; clip + Adam read them (no separate sum-of-squares launch)
+      rc = minibatch_fwdbwd(&a, stream, true);
       if (rc) return rc;
-      const PpoLayout La = make_layout(a.dims);
-      const TrainPlan Pa = plan_train(a.dims, std::max<int64_t>(a.m, 1));
-      AdamP ap = make_adam_params(&a, La, Pa);
-      ap.norm_partials = ws_ptr<float>(a.workspace, Pa.off_barrier) + 4;
-      ap.nblk_norm = 1;
-      RLX_LAUNCH_C(KC_CLIP_ADAM, 0, 28.0 * La.total(), ppo_clip_adam_kernel, (unsigned)ceil_div(La.total(), 256), 256, 0, st, ap);
-      continue;
-    }
-    if (!fused || a.m != std::min<int64_t>(mb, count)) {  // a short last minibatch has its own workspace plan: separate kernels
-      int rc = rlx_ppo_minibatch_fwdbwd_f32(&a, stream);
+      rc = launch_clip_adam(&a, make_layout(a.dims), ws_ptr<float>(a.workspace, P.off_barrier) + 4, 1, st);
+    } else {
+      // no optimiser state, or the short last minibatch (its workspace plan puts the ticket word elsewhere, not zeroed above):
+      // separate sum-of-squares launch
+      rc = minibatch_fwdbwd(&a, stream);
       if (rc) return rc;
       rc = rlx_gradnorm_clip_adam_f32(&a, stream);
-      if (rc) return rc;
-      continue;
     }
-    TailP t{};
-    int rc = minibatch_fwdbwd(&a, stream, &t.r);
     if (rc) return rc;
-    if (tall_elements(t.r) > 2LL * tail_grid * (kTailThreads / 32)) {  // more per-CTA partial columns than two per warp: separate kernels
-      rc = launch_grad_reduce(t.r, st);
-      if (rc) return rc;
-      rc = rlx_gradnorm_clip_adam_f32(&a, stream);
-      if (rc) return rc;
-      continue;
-    }
-    const TrainPlan P = plan_train(a.dims, std::max<int64_t>(a.m, 1));
-    t.a = make_adam_params(&a, L, P);
-    t.a.nblk_norm = (int)tail_grid;
-    t.barrier = ws_ptr<unsigned int>(a.workspace, P.off_barrier);
-    RLX_LAUNCH_C(KC_CLIP_ADAM, 0, partial_bytes(t.r) + 28.0 * L.total(), ppo_fused_tail_kernel, tail_grid, kTailThreads, 0, st, t);
   }
   return RLX_OK;
 }
@@ -732,44 +729,34 @@ extern "C" int rlx_ppo_update_epoch_sharded_f32(const rlx_ppo_minibatch_args* fi
                                                 const int64_t* global_counts, rlx_comm* comm, void* stream) {
   RLX_CHECK_ARG(first != nullptr && num_mb >= 0 && counts && global_counts && comm, "bad arguments");
   RLX_CHECK_ARG(first->metrics != nullptr, "metrics rows are required");
-  const int A = first->dims.act_dim;
-  const int64_t O = first->states_ld > 0 ? first->states_ld : first->dims.obs_dim;
-  const int64_t P = make_layout(first->dims).total();
+  const PpoLayout L = make_layout(first->dims);
+  const int64_t P = L.total();
   cudaStream_t st = (cudaStream_t)stream;
   int64_t r0 = 0;
   for (int64_t k = 0; k < num_mb; ++k) {
     RLX_CHECK_ARG(counts[k] >= 0 && global_counts[k] >= 1, "bad minibatch sizes");
-    rlx_ppo_minibatch_args a = *first;
-    a.m = counts[k];
+    rlx_ppo_minibatch_args a = minibatch_slice(first, k, r0, counts[k]);
     a.m_global = global_counts[k];
-    a.states = first->states + r0 * O;
-    a.actions = first->actions + r0 * A;
-    a.log_probs = first->log_probs + r0;
-    a.advantages = first->advantages + r0;
-    a.returns = first->returns + r0;
-    a.adv_stats = first->adv_stats + 2 * k;
     float* send = rlx_comm_send_buffer(comm);  // partial gradient [P] followed by the partial metric sums
     a.grads = send;
     a.metrics = send + P;
-    int rc = rlx_ppo_minibatch_fwdbwd_f32(&a, stream);
+    int rc = minibatch_fwdbwd(&a, stream);
     if (rc) return rc;
     // the two-shot exchange kernel leaves the per-net squared norms of the reduced gradient behind (and bumps Adam's step counter):
     // clip + Adam follow directly, without a separate pass over the gradient
-    const TrainPlan TP = plan_train(a.dims, std::max<int64_t>(a.m, 1));
+    float* norm_partials = ws_ptr<float>(a.workspace, plan_train(a.dims, std::max<int64_t>(a.m, 1)).off_norm);
     int nblk = 0;
-    rc = comm_allreduce_ppo(comm, first->grads, P + RLX_PPO_NMETRIC, a.dims, ws_ptr<float>(a.workspace, TP.off_norm), (long long*)a.step_count, stream, &nblk);
+    rc = comm_allreduce_ppo(comm, first->grads, P + RLX_PPO_NMETRIC, a.dims, norm_partials, (long long*)a.step_count, stream, &nblk);
     if (rc) return rc;
     a.grads = first->grads;
     a.metrics = first->grads + P;
     if (nblk > 0) {
       RLX_CHECK_ARG(a.exp_avg && a.exp_avg_sq && a.lr && a.step_count, "optimizer state is null");
-      AdamP ap = make_adam_params(&a, make_layout(a.dims), TP);
-      ap.nblk_norm = nblk;
-      RLX_LAUNCH_C(KC_CLIP_ADAM, 0, 28.0 * P, ppo_clip_adam_kernel, (unsigned)ceil_div(P, 256), 256, 0, st, ap);
+      rc = launch_clip_adam(&a, L, norm_partials, nblk, st);
     } else {
       rc = rlx_gradnorm_clip_adam_f32(&a, stream);  // writes the two pre-clip norms next to the summed metrics
-      if (rc) return rc;
     }
+    if (rc) return rc;
     RLX_CHECK_CUDA(cudaMemcpyAsync(first->metrics + RLX_PPO_NMETRIC * k, first->grads + P, RLX_PPO_NMETRIC * sizeof(float),
                                    cudaMemcpyDeviceToDevice, st));
     r0 += counts[k];
@@ -809,11 +796,6 @@ extern "C" int rlx_set_head_engine(int engine) {
   if (engine >= 0 && engine <= 2) g_head_engine = engine;
   else set_error("rlx_set_head_engine: unknown engine %d", engine);
   return g_head_engine;
-}
-
-extern "C" int rlx_set_fused_tail(int on) {
-  g_fused_tail = on ? 1 : 0;
-  return g_fused_tail;
 }
 
 extern "C" int rlx_set_gemm_engine(int engine) {

@@ -528,9 +528,7 @@ __global__ void __launch_bounds__(256, 2) ppo_head_train2_kernel(const HeadP p, 
   }
 }
 
-// ------------------------------------------------------- weight gradient of the head, fast variant (register tiled)
-// dW3 = dhead^T [act+1, M] . H2 [M, 2H].  Thread t owns policy columns {2t, 2t+1} and critic columns {H+2t, H+2t+1}
-// (64-bit coalesced loads); the act+1 gradient scalars of a row are broadcast from shared memory as float4.
+// ------------------------------------------------------- weight gradient of the head: dW3 = dhead^T [act+1, M] . H2 [M, 2H]
 // part[chunk][(act+1)*H]: rows 0..act-1 = dW3p, row act = dW3c.
 struct HeadWgrad2P {
   int M, H, act, dh_ld, rows_per_chunk;
@@ -538,55 +536,6 @@ struct HeadWgrad2P {
   const float* dhead;  // [M, dh_ld]
   float* part;
 };
-
-template <int ACT_MAX>  // multiple of 4, >= act + 1
-__global__ void __launch_bounds__(512) ppo_head_wgrad2_kernel(const HeadWgrad2P p) {
-  extern __shared__ __align__(16) float sd[];  // [rows_per_chunk][dh_ld]
-  const int chunk = blockIdx.x;
-  const long long r0 = (long long)chunk * p.rows_per_chunk;
-  const int nrows = (int)min((long long)p.rows_per_chunk, (long long)p.M - r0);
-  for (int i = threadIdx.x; i < nrows * p.dh_ld; i += blockDim.x) sd[i] = p.dhead[r0 * p.dh_ld + i];
-  __syncthreads();
-  const int t = threadIdx.x;
-  if (2 * t >= p.H) return;
-  float accp[ACT_MAX][2], accc[2] = {0.f, 0.f};
-#pragma unroll
-  for (int a = 0; a < ACT_MAX; ++a) accp[a][0] = accp[a][1] = 0.f;
-  const float* __restrict__ base = p.H2 + r0 * (2LL * p.H) + 2 * t;
-#pragma unroll 2
-  for (int r = 0; r < nrows; ++r) {
-    const float2 hpv = *reinterpret_cast<const float2*>(base + (long long)r * 2 * p.H);
-    const float2 hcv = *reinterpret_cast<const float2*>(base + (long long)r * 2 * p.H + p.H);
-    const float4* dr = reinterpret_cast<const float4*>(sd + r * p.dh_ld);
-    float d[ACT_MAX];
-#pragma unroll
-    for (int q = 0; q < ACT_MAX / 4; ++q) {
-      if (4 * q < p.dh_ld) {
-        const float4 v = dr[q];
-        d[4 * q] = v.x; d[4 * q + 1] = v.y; d[4 * q + 2] = v.z; d[4 * q + 3] = v.w;
-      } else {
-        d[4 * q] = d[4 * q + 1] = d[4 * q + 2] = d[4 * q + 3] = 0.f;
-      }
-    }
-    float dv = 0.f;
-#pragma unroll
-    for (int a = 0; a < ACT_MAX; ++a) {
-      if (a < p.act) {
-        accp[a][0] = fmaf(d[a], hpv.x, accp[a][0]);
-        accp[a][1] = fmaf(d[a], hpv.y, accp[a][1]);
-      } else if (a == p.act) {
-        dv = d[a];
-      }
-    }
-    accc[0] = fmaf(dv, hcv.x, accc[0]);
-    accc[1] = fmaf(dv, hcv.y, accc[1]);
-  }
-  float* out = p.part + (long long)chunk * (p.act + 1) * p.H + 2 * t;
-#pragma unroll
-  for (int a = 0; a < ACT_MAX; ++a)
-    if (a < p.act) *reinterpret_cast<float2*>(out + (long long)a * p.H) = make_float2(accp[a][0], accp[a][1]);
-  *reinterpret_cast<float2*>(out + (long long)p.act * p.H) = make_float2(accc[0], accc[1]);
-}
 
 // ------------------------------------------------------------ train head, vectorised variant (H multiple of 128)
 // Lane l owns the 4-column groups {g*128 + 4l .. +3}: H2 / dZ2 rows move as coalesced 128-bit accesses and every W3 fetch is
