@@ -450,6 +450,59 @@ int rlx_fastsac_act_f32(const rlx_fastsac_dims* d, const float* policy_params, c
 int rlx_fastsac_normalize_f32(const float* x, int64_t n, int64_t obs_dim, float* mean, float* var, float* std, int64_t* count, int32_t update,
                               float eps, float* out, float* workspace, void* stream);
 
+/* -------------------------------------------------------------------------------------------- FastTD3 update -- */
+/* rl_x/algorithms/fasttd3/pytorch, fp32 path.  Numerics are also checked by running these sources in a host emulation build against
+ * oracle/fasttd3_oracle.py, which is pinned to the executed reference (tests/test_fasttd3_emulation.py); GPU tests:
+ * tests/test_gpu_zzzzz_fasttd3.py.  The C51 critic machinery (projection, cross-entropy, AdamW, polyak) is FastSAC's (csrc/c51_ops.cuh).
+ * Networks (fixed widths like the reference): policy Linear-ReLU x3 (512, 256, 128) + Linear(act) + tanh (policy.py:33-42);
+ * Q network Linear-ReLU x3 (1024, 512, 256) + nr_atoms logits on [state | action] (q_network.py:27-35).
+ * Flat parameter layouts, torch [out, in] weights in state_dict order:  (W, b) x 4  -> 8 segments each; q buffers hold q1 | q2, the target
+ * buffer q1_target | q2_target.  Dense layers go through the aux GEMM engine (rlx_set_aux_gemm_engine). */
+#define RLX_FASTTD3_POLICY_NSEG 8
+#define RLX_FASTTD3_Q_NSEG 8
+typedef struct rlx_fasttd3_dims { int32_t obs_dim, act_dim, nr_atoms; } rlx_fasttd3_dims;
+int rlx_fasttd3_param_layout(const rlx_fasttd3_dims* d, int64_t* policy_offsets /*[9]*/, int64_t* q_offsets /*[9], one network*/);
+size_t rlx_fasttd3_workspace_bytes(const rlx_fasttd3_dims* d, int64_t n);
+
+typedef struct rlx_fasttd3_hparams {
+  float gamma, tau, v_min, v_max, smoothing_epsilon, smoothing_clip_value;
+  float weight_decay, adam_beta1, adam_beta2, adam_eps, max_grad_norm;  /* max_grad_norm < 0: no clipping (fasttd3.py:125-132) */
+  float clipped_double_q;           /* != 0: both critics learn the target distribution of the smaller next value, the actor maximises
+                                       min(q1, q2) (fasttd3.py:115-118,191-197) */
+} rlx_fasttd3_hparams;
+
+typedef struct rlx_fasttd3_update_args {
+  rlx_fasttd3_dims dims;
+  int64_t n;                        /* batch rows */
+  const float* states;              /* [n, obs] normalised */
+  const float* next_states;         /* [n, obs] normalised (critic update only) */
+  const float* actions;             /* [n, act] (critic update only) */
+  const float* rewards;             /* [n] n-step rewards */
+  const float* dones;               /* [n] */
+  const float* truncations;         /* [n] */
+  const float* effective_n_steps;   /* [n] */
+  const float* smoothing_noise;     /* [n, act] standard normal draws of the target-policy smoothing (critic update only) */
+  float* policy_params;  float* policy_grads;  float* policy_m;  float* policy_v;
+  float* q_params;       float* q_grads;       float* q_m;       float* q_v;        /* q1 | q2 */
+  float* q_target_params;                                                           /* q1_target | q2_target */
+  const float* lr;                  /* [1] device */
+  int64_t* steps;                   /* [2] device: q, policy optimiser step counters */
+  rlx_fasttd3_hparams hp;
+  float* metrics;                   /* critic update: q_loss, q_min, q_max, critic_grad_norm; policy update: policy_loss, policy_grad_norm */
+  void* workspace;
+  size_t workspace_bytes;
+} rlx_fasttd3_update_args;
+/* ref: critic_loss_fn + its optimiser step (fasttd3.py:139-225) + the polyak update that follows it (:316-320).  The target actions come
+ * from the ONLINE policy: clamp(policy(s') + clamp(smoothing_epsilon * noise, +-clip), -1, 1) (:143-144) */
+int rlx_fasttd3_critic_update_f32(const rlx_fasttd3_update_args* a, void* stream);
+/* ref: policy_loss_fn + optimiser step (fasttd3.py:104-136) */
+int rlx_fasttd3_policy_update_f32(const rlx_fasttd3_update_args* a, void* stream);
+/* ref: Policy.get_action (policy.py:57-66): action = tanh_mlp(obs) + noise * noise_scale[row]; noise NULL: deterministic (noise_scale unused).
+ * env_action (nullable) = low + 0.5 (clamp(action, -1, 1) + 1) (high - low) when clip_rescale != 0, else the action.  workspace as above */
+int rlx_fasttd3_act_f32(const rlx_fasttd3_dims* d, const float* policy_params, const float* obs, const float* noise, const float* noise_scale,
+                        const float* act_low, const float* act_high, int32_t clip_rescale, int64_t n, float* action, float* env_action, void* workspace,
+                        size_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------------- SAC path -- */
 /* ref: ReplayBuffer.sample gathers  (sac/pytorch/replay_buffer.py:32-40):  rows states[idx1, idx2] etc. from the device ring.
  * ring arrays are [capacity_per_env, nr_envs, dim]; idx_t/idx_e [n] int64. */

@@ -143,6 +143,25 @@ class FastSacUpdateArgs(C.Structure):
                                            "q_target_params", "log_alpha", "alpha_state", "lr", "steps")] +
                 [("hp", FastSacHparams), ("metrics", C.c_void_p), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)])
 
+RLX_FASTTD3_POLICY_NSEG, RLX_FASTTD3_Q_NSEG = 8, 8
+
+
+class FastTd3Dims(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("obs_dim", "act_dim", "nr_atoms")]
+
+
+class FastTd3Hparams(C.Structure):
+    _fields_ = [(n, C.c_float) for n in ("gamma", "tau", "v_min", "v_max", "smoothing_epsilon", "smoothing_clip_value", "weight_decay", "adam_beta1",
+                                         "adam_beta2", "adam_eps", "max_grad_norm", "clipped_double_q")]
+
+
+class FastTd3UpdateArgs(C.Structure):
+    _fields_ = ([("dims", FastTd3Dims), ("n", C.c_int64)] +
+                [(k, C.c_void_p) for k in ("states", "next_states", "actions", "rewards", "dones", "truncations", "effective_n_steps", "smoothing_noise",
+                                           "policy_params", "policy_grads", "policy_m", "policy_v", "q_params", "q_grads", "q_m", "q_v",
+                                           "q_target_params", "lr", "steps")] +
+                [("hp", FastTd3Hparams), ("metrics", C.c_void_p), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)])
+
 RLX_SAC_NMETRIC = 12
 RLX_COMM_MAX_WORLD = 16
 RLX_COMM_HANDLE_BYTES = 64
@@ -194,6 +213,12 @@ _SIGNATURES = {
                                       C.c_void_p, C.c_size_t, C.c_void_p]),
     "rlx_fastsac_normalize_f32": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_float,
                                             C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rlx_fasttd3_param_layout": (C.c_int, [C.POINTER(FastTd3Dims), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "rlx_fasttd3_workspace_bytes": (C.c_size_t, [C.POINTER(FastTd3Dims), C.c_int64]),
+    "rlx_fasttd3_critic_update_f32": (C.c_int, [C.POINTER(FastTd3UpdateArgs), C.c_void_p]),
+    "rlx_fasttd3_policy_update_f32": (C.c_int, [C.POINTER(FastTd3UpdateArgs), C.c_void_p]),
+    "rlx_fasttd3_act_f32": (C.c_int, [C.POINTER(FastTd3Dims)] + [C.c_void_p] * 6 + [C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                      C.c_void_p]),
     "rlx_ppo_param_count": (C.c_int64, [C.POINTER(PpoDims)]),
     "rlx_ppo_param_layout": (C.c_int, [C.POINTER(PpoDims), C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
     "rlx_ppo_forward_workspace_bytes": (C.c_size_t, [C.POINTER(PpoDims), C.c_int64]),

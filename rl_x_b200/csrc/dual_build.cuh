@@ -76,6 +76,8 @@ int launch_sgemm(const GemmP& p, int batch, cudaStream_t, int = 0, long long a_r
         if (EPI == EPI_BIAS) acc += p.bias[b * p.sBias + n];
         if (EPI == EPI_BIAS_TANH) acc = tanhf(acc + p.bias[b * p.sBias + n]);
         if (EPI == EPI_DTANH) { const float h = p.aux[b * p.sAux + (long long)m * p.ldaux + n]; acc = acc * (1.f - h * h); }
+        if (EPI == EPI_BIAS_RELU) acc = fmaxf(acc + p.bias[b * p.sBias + n], 0.f);
+        if (EPI == EPI_DRELU) { const float h = p.aux[b * p.sAux + (long long)m * p.ldaux + n]; acc = h > 0.f ? acc : 0.f; }
         C[(long long)m * p.ldc + n] = acc;
       }
   }

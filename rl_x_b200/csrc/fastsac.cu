@@ -2,17 +2,17 @@
 // coefficient, AdamW, polyak targets, observation normaliser.  Entry points and flat layouts: include/rlx_b200.h.
 // Dual build (dual_build.cuh): the host emulation of this file is checked against oracle/fastsac_oracle.py (pinned to the executed
 // reference) in tests/test_fastsac_emulation.py.  v1: exact-fp32 SIMT GEMMs, flat one-thread-per-row / per-element kernels.
-#include "flat_ops.cuh"
+#include "c51_ops.cuh"
 
 namespace rlx {
 namespace fsac {
 using namespace rlx::flat;
+using namespace rlx::c51;
 
 constexpr int kPW[3] = {512, 256, 128};   // policy torso widths (policy.py:36-46)
 constexpr int kQW[3] = {768, 384, 192};   // Q torso widths (q_network.py:24-34)
 constexpr float kLnEps = 1e-5f;           // torch.nn.LayerNorm default
 constexpr float kHalfLog2Pi = 0.9189385332046727f;
-constexpr int kWgradRows = 1024;
 
 struct Layout {
   long long p[RLX_FASTSAC_POLICY_NSEG + 1], q[RLX_FASTSAC_Q_NSEG + 1];
@@ -136,15 +136,6 @@ __global__ void ln_silu_param_partial_kernel(const float* __restrict__ dOut, con
   part_g[id] = sg;
   part_b[id] = sb;
 }
-// XA = [X | A]  thread = element
-__global__ void concat_kernel(const float* __restrict__ X, const float* __restrict__ A, long long n, int O, int Ad, float* __restrict__ XA) {
-  const long long id = gtid();
-  const int W = O + Ad;
-  if (id >= n * W) return;
-  const long long r = id / W;
-  const int k = (int)(id % W);
-  XA[id] = k < O ? X[r * O + k] : A[r * Ad + (k - O)];
-}
 // policy head: tanh log-std squash, reparameterised sample, tanh action, log-prob with the squash / scale corrections (policy.py:55-75).
 // noise == null: deterministic action tanh(mean) * scale.  thread = row
 __global__ void squash_sample_kernel(const float* __restrict__ Mean, const float* __restrict__ LsRaw, const float* __restrict__ noise,
@@ -187,124 +178,9 @@ __global__ void squash_sample_bwd_kernel(const float* __restrict__ Mean, const f
     dLs[r * A + a] = dls * 0.5f * (lsmax - lsmin) * (1.f - tl * tl);
   }
 }
-// dAct[r, a] = dXA0[r, O + a] + dXA1[r, O + a]: the action columns of the two critics' input gradients.  thread = element
-__global__ void action_grad_kernel(const float* __restrict__ dXA0, const float* __restrict__ dXA1, long long n, int O, int A, float* __restrict__ dAct) {
-  const long long id = gtid();
-  if (id >= n * A) return;
-  const long long r = id / A;
-  const int a = (int)(id % A);
-  dAct[id] = dXA0[r * (O + A) + O + a] + dXA1[r * (O + A) + O + a];
-}
 __global__ void add_inplace_kernel(float* __restrict__ x, const float* __restrict__ y, long long n) {
   const long long i = gtid();
   if (i < n) x[i] += y[i];
-}
-// expected value of softmax(logits) on the support; optionally the gradient of (-coef * value) wrt the logits.  thread = row
-__global__ void expect_rows_kernel(const float* __restrict__ logits, long long n, int K, float v_min, float v_max, float* __restrict__ value,
-                                   float coef, float* __restrict__ dlogits) {
-  const long long r = gtid();
-  if (r >= n) return;
-  const float* l = logits + r * K;
-  float mx = l[0];
-  for (int k = 1; k < K; ++k) mx = fmaxf(mx, l[k]);
-  float den = 0.f;
-  for (int k = 0; k < K; ++k) den += expf(l[k] - mx);
-  const float dz = (v_max - v_min) / (float)(K - 1);
-  float v = 0.f;
-  for (int k = 0; k < K; ++k) v += expf(l[k] - mx) / den * (v_min + dz * (float)k);
-  value[r] = v;
-  if (dlogits)
-    for (int k = 0; k < K; ++k) {
-      const float p = expf(l[k] - mx) / den;
-      dlogits[r * K + k] = coef * p * ((v_min + dz * (float)k) - v);
-    }
-}
-// gradient of -mean(q) wrt one critic's logits, q = (v1 + v2) / 2 or min(v1, v2) (ties split evenly like torch.minimum).  thread = row
-__global__ void value_grad_rows_kernel(const float* __restrict__ logits, const float* __restrict__ v_self, const float* __restrict__ v_other,
-                                       long long n, int K, float v_min, float v_max, int clipped, float inv_n, float* __restrict__ dlogits) {
-  const long long r = gtid();
-  if (r >= n) return;
-  const float vs = v_self[r], vo = v_other[r];
-  const float coef = clipped ? (vs < vo ? 1.f : (vs == vo ? 0.5f : 0.f)) : 0.5f;
-  const float* l = logits + r * K;
-  float mx = l[0];
-  for (int k = 1; k < K; ++k) mx = fmaxf(mx, l[k]);
-  float den = 0.f;
-  for (int k = 0; k < K; ++k) den += expf(l[k] - mx);
-  const float dz = (v_max - v_min) / (float)(K - 1);
-  for (int k = 0; k < K; ++k) dlogits[r * K + k] = -coef * inv_n * (expf(l[k] - mx) / den) * ((v_min + dz * (float)k) - vs);
-}
-__global__ void combine_values_kernel(const float* __restrict__ v1, const float* __restrict__ v2, long long n, int clipped, float* __restrict__ out) {
-  const long long r = gtid();
-  if (r >= n) return;
-  out[r] = clipped ? fminf(v1[r], v2[r]) : (v1[r] + v2[r]) / 2.f;
-}
-// C51 target of one row (fastsac.py:146-186): both target distributions are projected with the same bins.  thread = row
-__global__ void c51_project_kernel(const float* __restrict__ tl1, const float* __restrict__ tl2, const float* __restrict__ rewards,
-                                   const float* __restrict__ dones, const float* __restrict__ truncs, const float* __restrict__ eff,
-                                   const float* __restrict__ next_logp, const float* __restrict__ log_alpha, long long n, int K, float gamma,
-                                   float v_min, float v_max, int clipped, float* __restrict__ proj1, float* __restrict__ proj2,
-                                   float* __restrict__ q1_next_value) {
-  const long long r = gtid();
-  if (r >= n) return;
-  const float dz = (v_max - v_min) / (float)(K - 1);
-  const float bootstrap = 1.f - dones[r] * (1.f - truncs[r]);
-  const float discount = powf(gamma, eff[r]) * bootstrap;
-  const float adj = rewards[r] - discount * expf(log_alpha[0]) * next_logp[r];
-  float m1 = tl1[r * K], m2 = tl2[r * K];
-  for (int k = 1; k < K; ++k) { m1 = fmaxf(m1, tl1[r * K + k]); m2 = fmaxf(m2, tl2[r * K + k]); }
-  float d1 = 0.f, d2 = 0.f;
-  for (int k = 0; k < K; ++k) { d1 += expf(tl1[r * K + k] - m1); d2 += expf(tl2[r * K + k] - m2); }
-  for (int k = 0; k < K; ++k) { proj1[r * K + k] = 0.f; proj2[r * K + k] = 0.f; }
-  for (int k = 0; k < K; ++k) {
-    const float z = fminf(fmaxf(adj + discount * (v_min + dz * (float)k), v_min), v_max);
-    const float b = (z - v_min) / dz;
-    int lo = (int)floorf(b), up = (int)ceilf(b);
-    if (lo == up) {  // b on a bin: move one neighbour so that the two weights still sum to 1 (:155-160)
-      if (lo > 0) lo -= 1; else up += 1;
-    }
-    const float wl = (float)up - b, wu = b - (float)lo;
-    const float p1 = expf(tl1[r * K + k] - m1) / d1, p2 = expf(tl2[r * K + k] - m2) / d2;
-    proj1[r * K + lo] += p1 * wl; proj1[r * K + up] += p1 * wu;
-    proj2[r * K + lo] += p2 * wl; proj2[r * K + up] += p2 * wu;
-  }
-  float v = 0.f, v2 = 0.f;
-  for (int k = 0; k < K; ++k) { v += proj1[r * K + k] * (v_min + dz * (float)k); v2 += proj2[r * K + k] * (v_min + dz * (float)k); }
-  q1_next_value[r] = v;
-  if (clipped) {  // torch.where(q1_next < q2_next, proj1, proj2) for BOTH critics (fastsac.py:179-182)
-    for (int k = 0; k < K; ++k) {
-      const float sel = (v < v2) ? proj1[r * K + k] : proj2[r * K + k];
-      proj1[r * K + k] = sel;
-      proj2[r * K + k] = sel;
-    }
-  }
-}
-// cross-entropy of one row against its projected target: loss = -sum_k proj_k log_softmax(logits)_k; dlogits = (softmax * sum(proj) - proj) / n
-__global__ void ce_rows_kernel(const float* __restrict__ logits, const float* __restrict__ proj, long long n, int K, float inv_n,
-                               float* __restrict__ loss_row, float* __restrict__ dlogits) {
-  const long long r = gtid();
-  if (r >= n) return;
-  const float* l = logits + r * K;
-  float mx = l[0];
-  for (int k = 1; k < K; ++k) mx = fmaxf(mx, l[k]);
-  float den = 0.f;
-  for (int k = 0; k < K; ++k) den += expf(l[k] - mx);
-  const float lse = mx + logf(den);
-  float loss = 0.f, ps = 0.f;
-  for (int k = 0; k < K; ++k) { loss -= proj[r * K + k] * (l[k] - lse); ps += proj[r * K + k]; }
-  for (int k = 0; k < K; ++k) dlogits[r * K + k] = (expf(l[k] - lse) * ps - proj[r * K + k]) * inv_n;
-  loss_row[r] = loss;
-}
-// rows -> (min, max) per chunk, then one thread finishes.
-__global__ void minmax_partial_kernel(const float* __restrict__ x, long long n, float* __restrict__ part) {
-  const long long c = gtid();
-  const long long nchunk = (n + kColChunk - 1) / kColChunk;
-  if (c >= nchunk) return;
-  const long long r1 = c * kColChunk + kColChunk < n ? c * kColChunk + kColChunk : n;
-  float lo = x[c * kColChunk], hi = lo;
-  for (long long r = c * kColChunk + 1; r < r1; ++r) { lo = fminf(lo, x[r]); hi = fmaxf(hi, x[r]); }
-  part[2 * c] = lo;
-  part[2 * c + 1] = hi;
 }
 // critic metrics + the entropy-coefficient gradient (fastsac.py:228-236).  sums: [sum loss1, sum loss2, sum next_logp]
 __global__ void critic_finish_kernel(const float* __restrict__ sums, const float* __restrict__ mm_part, long long nchunk, float n,
@@ -328,29 +204,6 @@ __global__ void policy_finish_kernel(const float* __restrict__ sums, float n, co
   const float al = expf(log_alpha[0]);
   metrics[0] = al * sums[0] / n - sums[1] / n;  // mean(alpha * logp - q), q = (q1 + q2) / 2 or min(q1, q2)
   metrics[1] = al;
-}
-// torch.optim.AdamW (single tensor): p *= 1 - lr wd; m, v updates; p -= lr / bc1 * m / (sqrt(v) / sqrt(bc2) + eps).  Optional clip_grad_norm_.
-__global__ void adamw_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, long long n,
-                             const float* __restrict__ lr, const long long* __restrict__ step, const float* __restrict__ norm, float max_norm,
-                             float wd, float b1, float b2, float eps) {
-  const long long i = gtid();
-  if (i >= n) return;
-  float gi = g[i];
-  if (max_norm >= 0.f) gi *= fminf(1.f, max_norm / (norm[0] + 1e-6f));
-  const float t = (float)step[0];
-  float pi = p[i] * (1.f - lr[0] * wd);
-  const float mi = b1 * m[i] + (1.f - b1) * gi;
-  const float vi = b2 * v[i] + (1.f - b2) * gi * gi;
-  m[i] = mi;
-  v[i] = vi;
-  const float bc1 = 1.f - powf(b1, t), bc2 = 1.f - powf(b2, t);
-  pi -= lr[0] / bc1 * mi / (sqrtf(vi) / sqrtf(bc2) + eps);
-  p[i] = pi;
-}
-__global__ void polyak_kernel(float* __restrict__ tgt, const float* __restrict__ src, long long n, float tau) {
-  const long long i = gtid();
-  if (i >= n) return;
-  tgt[i] = tgt[i] * (1.f - tau) + tau * src[i];
 }
 // observation normaliser: batch column mean / biased variance from partials, Chan's update (observation_normalizer.py:28-47).  thread = column
 __global__ void normalizer_update_kernel(const float* __restrict__ col_sum, const float* __restrict__ col_sq, long long n, int O,
@@ -384,36 +237,6 @@ __global__ void normalize_kernel(const float* __restrict__ x, long long n, int O
   if (id >= n * O) return;
   const int j = (int)(id % O);
   out[id] = (x[id] - mean[j]) / (stdv[j] + eps);
-}
-
-// ------------------------------------------------------------------------------------------------------- GEMM helpers
-// torch Linear: Y[r, o] = sum_i X[r, i] W[o, i] + b[o]
-static int lin_fwd(const float* X, int ldx, const float* W, int in, int out, const float* b, float* Y, int ldy, long long n, cudaStream_t st) {
-  GemmP g{};
-  g.A = X; g.B = W; g.C = Y; g.bias = b;
-  g.M = (int)n; g.N = out; g.K = in; g.lda = ldx; g.ldb = in; g.ldc = ldy;
-  g.splits = 1; g.kchunk = (int)(ceil_div(in, 8) * 8);
-  return aux_gemm<true, true, EPI_BIAS>(g, 1, st, KC_GEMM_FWD, n, out);
-}
-// dX[r, i] = sum_o dY[r, o] W[o, i]
-static int lin_bwd_input(const float* dY, int ldy, const float* W, int in, int out, float* dX, int ldx, long long n, cudaStream_t st) {
-  GemmP g{};
-  g.A = dY; g.B = W; g.C = dX;
-  g.M = (int)n; g.N = in; g.K = out; g.lda = ldy; g.ldb = in; g.ldc = ldx;
-  g.splits = 1; g.kchunk = (int)(ceil_div(out, 8) * 8);
-  return aux_gemm<true, false, EPI_NONE>(g, 1, st, KC_GEMM_DX, n, out);
-}
-// dW[o, i] = sum_r dY[r, o] X[r, i], split over rows
-static int lin_bwd_weight(const float* dY, int ldy, const float* X, int ldx, int in, int out, long long n, float* part, float* dW, cudaStream_t st) {
-  const int splits = (int)ceil_div(n, kWgradRows);
-  GemmP g{};
-  g.A = dY; g.B = X; g.C = part;
-  g.M = out; g.N = in; g.K = (int)n; g.lda = ldy; g.ldb = ldx; g.ldc = in;
-  g.splits = splits; g.kchunk = kWgradRows; g.sSplitC = (long long)in * out;
-  int rc = aux_gemm<false, false, EPI_NONE>(g, 1, st, KC_GEMM_DW, n, n);
-  if (rc) return rc;
-  RLX_FLAT_LAUNCH(reduce_parts_kernel, (long long)in * out, st, part, (long long)splits, (long long)in * out, 1.f, 0.f, dW);
-  return RLX_OK;
 }
 
 #define FS_TRY(expr) do { int _rc = (expr); if (_rc) return _rc; } while (0)
@@ -482,12 +305,7 @@ static int q_bwd(const rlx_fastsac_dims& d, const Layout& l, const Ws& w, float*
 }
 static int adamw(float* p, const float* g, float* m, float* v, long long n, const float* lr, long long* step, const rlx_fastsac_hparams& hp,
                  float* norm_out, float* scratch, cudaStream_t st) {
-  const long long nchunk = ceil_div(n, 1024);
-  RLX_FLAT_LAUNCH(sumsq_partial_kernel, nchunk, st, g, n, scratch);
-  RLX_FLAT_LAUNCH(sumsq_final_kernel, 1, st, scratch, nchunk, norm_out, step);
-  RLX_FLAT_LAUNCH(adamw_kernel, n, st, p, g, m, v, n, lr, (const long long*)step, norm_out, hp.max_grad_norm, hp.weight_decay, hp.adam_beta1,
-                  hp.adam_beta2, hp.adam_eps);
-  return RLX_OK;
+  return adamw_step(p, g, m, v, n, lr, step, hp.max_grad_norm, hp.weight_decay, hp.adam_beta1, hp.adam_beta2, hp.adam_eps, norm_out, scratch, st);
 }
 
 }  // namespace fsac
@@ -537,7 +355,7 @@ extern "C" int rlx_fastsac_critic_update_f32(const rlx_fastsac_update_args* a, v
   const Acts q0 = acts_q(ws, w, 0), q1 = acts_q(ws, w, 1);
   // ---- target (no gradients): a' ~ pi(s'), both target networks on (s', a'), projection (fastsac.py:143-186)
   FS_TRY(policy_fwd(d, l, w, ws, a->policy_params, a->next_states, a->noise, a->action_scale, hp.log_std_min, hp.log_std_max, n, Act, Logp, st));
-  RLX_FLAT_LAUNCH(concat_kernel, n * (O + A), st, a->next_states, Act, n, O, A, XA);
+  RLX_FLAT_LAUNCH(concat_kernel, n * (O + A), st, a->next_states, Act, n, O, A, O + A, XA);
   FS_TRY(q_fwd(d, l, a->q_target_params, XA, n, q0, ws + w.Logits[0], st));
   FS_TRY(q_fwd(d, l, a->q_target_params + nq, XA, n, q1, ws + w.Logits[1], st));
   RLX_FLAT_LAUNCH(c51_project_kernel, n, st, ws + w.Logits[0], ws + w.Logits[1], a->rewards, a->dones, a->truncations, a->effective_n_steps, Logp,
@@ -546,7 +364,7 @@ extern "C" int rlx_fastsac_critic_update_f32(const rlx_fastsac_update_args* a, v
   const long long nchunk = ceil_div(n, kColChunk);
   RLX_FLAT_LAUNCH(minmax_partial_kernel, nchunk, st, RowA, n, RowB);
   // ---- current critics on (s, a): cross-entropy and its gradient (fastsac.py:188-196)
-  RLX_FLAT_LAUNCH(concat_kernel, n * (O + A), st, a->states, a->actions, n, O, A, XA);
+  RLX_FLAT_LAUNCH(concat_kernel, n * (O + A), st, a->states, a->actions, n, O, A, O + A, XA);
   const float inv_n = 1.f / (float)n;
   for (int q = 0; q < 2; ++q) {
     const Acts& aq = q == 0 ? q0 : q1;
@@ -586,7 +404,7 @@ extern "C" int rlx_fastsac_policy_update_f32(const rlx_fastsac_update_args* a, v
   const float inv_n = 1.f / (float)n;
   // a ~ pi(s); q = (E[q1] + E[q2]) / 2 on (s, a); L = mean(alpha logp - q)   (fastsac.py:108-124)
   FS_TRY(policy_fwd(d, l, w, ws, a->policy_params, a->states, a->noise, a->action_scale, hp.log_std_min, hp.log_std_max, n, Act, Logp, st));
-  RLX_FLAT_LAUNCH(concat_kernel, n * (O + A), st, a->states, Act, n, O, A, XA);
+  RLX_FLAT_LAUNCH(concat_kernel, n * (O + A), st, a->states, Act, n, O, A, O + A, XA);
   const int clipped = hp.clipped_double_q != 0.f ? 1 : 0;
   for (int q = 0; q < 2; ++q) {
     FS_TRY(q_fwd(d, l, a->q_params + q * nq, XA, n, acts_q(ws, w, q), ws + w.Logits[q], st));
@@ -607,7 +425,7 @@ extern "C" int rlx_fastsac_policy_update_f32(const rlx_fastsac_update_args* a, v
     }
   }
   // dAct = action columns of both critics' input gradients; back through the squashed-Gaussian head and the policy torso
-  RLX_FLAT_LAUNCH(action_grad_kernel, n * A, st, dXA, ws + w.dXA2, n, O, A, dAct);
+  RLX_FLAT_LAUNCH(action_grad_kernel, n * A, st, dXA, ws + w.dXA2, n, O, A, O + A, dAct);
   RLX_FLAT_LAUNCH(squash_sample_bwd_kernel, n, st, ws + w.Mean, ws + w.LsRaw, a->noise, a->action_scale, dAct, a->log_alpha, n, A, hp.log_std_min,
                   hp.log_std_max, inv_n, ws + w.dMean, ws + w.dLs);
   const float* P = a->policy_params;
