@@ -8,15 +8,19 @@
 // 3xTF32 does not) at one third of the TF32 tensor rate.
 //
 // Structure (one persistent CTA per SM, 384 threads = 3 warpgroups, static tile schedule, 128 x 128 output tiles):
-//   warpgroup 0   thread 0 issues cp.async.bulk.tensor 2-D tiles (SWIZZLE_128B) of raw fp32 A and B into a 3-stage ring, running ahead
-//                 of the conversion; all 128 threads then write the hi and lo tiles of both operands, K-major and 128-byte swizzled
-//                 (the only layout wgmma accepts for tf32), into a 2-stage operand ring and fence.proxy.async it for the tensor core
-//   warpgroups 1, 2   rows 0-63 / 64-127 of the tile: wgmma.mma_async m64n128k8 tf32 (3 per k-slice of 8), then the epilogue straight
-//                 from the accumulator registers: bias+tanh / tanh' / relu / plain, stores to C (or C^T)
+//   warpgroup 0   thread 0 issues cp.async.bulk.tensor 2-D tiles (SWIZZLE_128B) of raw fp32 A and B into a 3-stage ring; all 128 threads
+//                 then write the hi and lo tiles of B, K-major and 128-byte swizzled (the only shared-memory layout wgmma accepts for
+//                 tf32), into a 4-stage operand ring and fence.proxy.async it for the tensor core
+//   warpgroups 1, 2   rows 0-63 / 64-127 of the tile: read their A fragments straight from the raw stage, split them into hi / lo in
+//                 registers, and issue wgmma.mma_async m64n128k8 tf32 with A from registers (3 per k-slice of 8), keeping one half k-block
+//                 of MMAs in flight while the next half's fragments are loaded; then the epilogue straight from the accumulator registers: bias+tanh / tanh' /
+//                 relu / plain, stores to C (or C^T)
+// A raw slot is refilled once the converter has used its B and all 8 consumer warps hold its A in registers; an operand slot once the
+// wgmmas that read it have retired.
 // Operand layouts in global memory: K-major (row = m or n, 32 consecutive k = one 128-byte swizzle row) or MN-major (row = k, 32
 // consecutive m/n per 128-byte row; used by the weight-gradient GEMMs whose reduction runs over the minibatch rows).  The converter
-// transposes MN-major tiles to K-major.  Out-of-bounds parts of a box are zero-filled by TMA, so M / N / K tails need no special code
-// in the main loop.
+// transposes MN-major B tiles to K-major; the consumers' fragment reads transpose MN-major A.  Out-of-bounds parts of a box are
+// zero-filled by TMA, so M / N / K tails need no special code in the main loop.
 #include "gemm_dispatch.cuh"
 #include "gemm_tc_common.cuh"
 
@@ -29,13 +33,17 @@ struct Cfg {
   static constexpr int A_BYTES = BM * BK * 4;                   // 16 KB
   static constexpr int B_BYTES = BN * BK * 4;                   // 16 KB
   static constexpr int RAW_BYTES = A_BYTES + B_BYTES;           // raw stage: [A | B] as TMA wrote them
-  static constexpr int OP_BYTES = 2 * RAW_BYTES;                // operand stage: [hi A | hi B | lo A | lo B], K-major swizzled
-  static constexpr int RAW_STAGES = 3, OP_STAGES = 2;
+  static constexpr int OP_BYTES = 2 * B_BYTES;                  // operand stage: [hi B | lo B], K-major swizzled
+  // the consumers hold up to two operand slots (the k-block being issued and the one retiring), so 4 stages let the converter run two ahead
+  static constexpr int RAW_STAGES = 3, OP_STAGES = 4;
   static constexpr int SMEM_BYTES = RAW_STAGES * RAW_BYTES + OP_STAGES * OP_BYTES + 1024 /*barriers*/ + 1024 /*alignment slack*/;
+  // consumers: 2 x 64 accumulators + 2 half k-blocks x 16 A-fragment registers
+  static constexpr int PRODUCER_REGS = 56, CONSUMER_REGS = 224;
 };
 static_assert(Cfg::SMEM_BYTES <= 227 * 1024, "shared memory of one H100 block");
+static_assert(Cfg::PRODUCER_REGS * 128 + Cfg::CONSUMER_REGS * 256 <= 65536, "register file of one SM");
 
-// One operand tile (ROWS x BK) from its raw stage to K-major swizzled hi / lo tiles.  In the 128-byte swizzle every 16-byte chunk
+// One B tile (ROWS x BK) from its raw stage to K-major swizzled hi / lo tiles.  In the 128-byte swizzle every 16-byte chunk
 // (4 k-values) c of row r sits at r * 128 + ((c ^ (r & 7)) << 4).  Thread t of the warpgroup handles chunks t, t + 128, ...
 template <bool KMAJ, bool BF16, int ROWS>
 __device__ __forceinline__ void convert_tile(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int t) {
@@ -75,6 +83,52 @@ __device__ __forceinline__ void convert_tile(const uint8_t* raw, uint8_t* hi, ui
   }
 }
 
+// A fragments of one half k-block (k-slices 2 half, 2 half + 1) for one consumer thread, from the raw stage, split into hi / lo (the
+// same split as convert_tile).  The thread holds rows r0 and r0 + 8 (r0 = row within the tile, r0 % 8 = lane / 4) at
+// k = lane % 4 + 4 j, j = 4 half + jj: k-slice of the half jj / 2, fragment register 2 (jj & 1) + row (see wgmma_tf32_m64n128k8).
+template <bool KMAJ, bool BF16>
+__device__ __forceinline__ void load_a_frags(const uint8_t* raw, int r0, int lane, int half, uint32_t (&hi)[2][4], uint32_t (&lo)[2][4]) {
+  constexpr uint32_t HI = 0xFFFFE000u;
+  const int t4 = lane & 3;
+  uint32_t v[2][4];
+  if (KMAJ) {
+    // row r is one 128-byte swizzle row; chunk j sits at (j ^ (r & 7)): the 8 row groups of a warp hit 8 different chunks, no conflicts
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const uint8_t* row = raw + (r0 + 8 * r) * 128 + t4 * 4;
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) v[r][jj] = *reinterpret_cast<const uint32_t*>(row + (((4 * half + jj) ^ (r0 & 7)) << 4));
+    }
+  } else {
+    // BM / 32 boxes of [BK k-rows][32 m]: element (m, k) at box m / 32, k * 128 + ((((m & 31) >> 2) ^ (k & 7)) << 4) + (m & 3) * 4.
+    // Lanes 16-31 read the pair partner j ^ 1 first: without that, lanes l and l ^ 17 hit the same bank (2-way conflicts).
+    const int s = (lane >> 4) & 1;
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int m = r0 + 8 * r;
+      const uint8_t* box = raw + (m >> 5) * (BK * 128) + (m & 3) * 4;
+      const int mc = (m & 31) >> 2;
+#pragma unroll
+      for (int jj = 0; jj < 4; jj += 2) {
+        const int j = 4 * half + jj;
+        const int k0 = t4 + 4 * (j + s), k1 = t4 + 4 * (j + 1 - s);
+        const uint32_t x0 = *reinterpret_cast<const uint32_t*>(box + k0 * 128 + ((mc ^ (k0 & 7)) << 4));
+        const uint32_t x1 = *reinterpret_cast<const uint32_t*>(box + k1 * 128 + ((mc ^ (k1 & 7)) << 4));
+        v[r][jj] = s ? x1 : x0;
+        v[r][jj + 1] = s ? x0 : x1;
+      }
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r)
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+      const uint32_t h = v[r][jj] & HI;
+      hi[jj >> 1][2 * (jj & 1) + r] = h;
+      if (!BF16) lo[jj >> 1][2 * (jj & 1) + r] = __float_as_uint(__uint_as_float(v[r][jj]) - __uint_as_float(h));
+    }
+}
+
 // BF16: the bf16-autocast variant (single-pass MMAs on bf16-valued operands, bf16 roundings in the epilogue), a compile-time switch so that
 // the fp32-equivalent kernels carry none of it
 template <bool A_KMAJ, bool B_KMAJ, int EPI, bool BF16>
@@ -87,14 +141,18 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* ops = smem + RAW_STAGES * Cfg::RAW_BYTES;
   uint64_t* raw_full = reinterpret_cast<uint64_t*>(ops + OP_STAGES * Cfg::OP_BYTES);  // [RAW_STAGES]  TMA landed
-  uint64_t* op_full = raw_full + RAW_STAGES;                                          // [OP_STAGES]   hi / lo tiles written
+  uint64_t* raw_empty = raw_full + RAW_STAGES;                                        // [RAW_STAGES]  B converted, A in registers
+  uint64_t* op_full = raw_empty + RAW_STAGES;                                         // [OP_STAGES]   hi / lo B tiles written
   uint64_t* op_empty = op_full + OP_STAGES;                                           // [OP_STAGES]   wgmmas of the slot retired
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_b);
-    for (int s = 0; s < RAW_STAGES; ++s) mbar_init(&raw_full[s], 1);
+    for (int s = 0; s < RAW_STAGES; ++s) {
+      mbar_init(&raw_full[s], 1);
+      mbar_init(&raw_empty[s], 1 + 8);  // the converter + one arrival per consumer warp
+    }
     for (int s = 0; s < OP_STAGES; ++s) {
       mbar_init(&op_full[s], 1);
       mbar_init(&op_empty[s], 8);  // one arrival per consumer warp
@@ -118,9 +176,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
   };
 
   if (warp < 4) {
-    // ===================================================== TMA (thread 0) + hi / lo converter (warpgroup 0)
+    // ===================================================== TMA (thread 0) + B hi / lo converter (warpgroup 0)
+    setmaxnreg_dec<Cfg::PRODUCER_REGS>();
     const int t = threadIdx.x;
-    // load cursor: the k-blocks of this CTA's tiles in consumption order; a raw slot is refilled as soon as the converter is done with it
+    // load cursor: the k-blocks of this CTA's tiles in consumption order; a raw slot is refilled once its raw_empty phase completes
     int ld_tile = blockIdx.x, ld_kb = 0, ld_count = 0;
     auto load_next = [&]() {
       while (ld_tile < num_tiles) {
@@ -132,6 +191,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
           continue;
         }
         const int slot = ld_count % RAW_STAGES;
+        mbar_wait(&raw_empty[slot], ((ld_count / RAW_STAGES) & 1) ^ 1);  // the first round passes: a fresh barrier's previous phase
         uint8_t* sa = smem + slot * Cfg::RAW_BYTES;
         uint8_t* sb = sa + Cfg::A_BYTES;
         uint64_t* bar = &raw_full[slot];
@@ -158,21 +218,24 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
       for (int i = 0; i < RAW_STAGES; ++i) load_next();
     int rs = 0, os = 0;
     uint32_t rph = 0, oph = 0;
+    bool refill = false;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int zb, zs, m0, n0, kbeg, nkb;
       tile_coords(tile, zb, zs, m0, n0, kbeg, nkb);
       for (int kb = 0; kb < nkb; ++kb) {
         mbar_wait(&raw_full[rs], rph);
         mbar_wait(&op_empty[os], oph ^ 1);
-        const uint8_t* raw = smem + rs * Cfg::RAW_BYTES;
         uint8_t* op = ops + os * Cfg::OP_BYTES;
-        convert_tile<A_KMAJ, BF16, BM>(raw, op, op + Cfg::RAW_BYTES, t);
-        convert_tile<B_KMAJ, BF16, BN>(raw + Cfg::A_BYTES, op + Cfg::A_BYTES, op + Cfg::RAW_BYTES + Cfg::A_BYTES, t);
+        convert_tile<B_KMAJ, BF16, BN>(smem + rs * Cfg::RAW_BYTES + Cfg::A_BYTES, op, op + Cfg::B_BYTES, t);
         fence_proxy_async();  // generic-proxy writes -> visible to the tensor core's async-proxy reads
         named_bar_sync(1, 128);  // the whole warpgroup is done with raw slot rs and has written operand slot os
         if (t == 0) {
           mbar_arrive(&op_full[os]);
-          load_next();  // refills raw slot rs
+          mbar_arrive(&raw_empty[rs]);
+          // refill the PREVIOUS k-block's raw slot: the consumers have usually taken its A by now, so this rarely waits, and the TMA
+          // still runs RAW_STAGES - 1 k-blocks ahead of the converter
+          if (refill) load_next();
+          refill = true;
         }
         if (++rs == RAW_STAGES) { rs = 0; rph ^= 1; }
         if (++os == OP_STAGES) { os = 0; oph ^= 1; }
@@ -180,44 +243,65 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
     }
   } else {
     // ===================================================== wgmma consumers + epilogue (warpgroups 1, 2)
+    setmaxnreg_inc<Cfg::CONSUMER_REGS>();
     const int cw = (warp >> 2) - 1;  // rows 64 * cw .. 64 * cw + 63 of the tile
+    const int r0 = cw * 64 + (warp & 3) * 16 + (lane >> 2);
     float acc[64], cor[64];
-    int os = 0;
-    uint32_t oph = 0;
+    // A fragments of the two half k-blocks that can be in flight: [half][k-slice of the half][register].  Each half is one commit group
+    // with registers of its own: a register operand must keep its value until its wgmma retires.
+    uint32_t ah[2][2][4], al[2][2][4];
+    int rs = 0, os = 0;
+    uint32_t rph = 0, oph = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int zb, zs, m0, n0, kbeg, nkb;
       tile_coords(tile, zb, zs, m0, n0, kbeg, nkb);
       for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait(&raw_full[rs], rph);
         mbar_wait(&op_full[os], oph);
+        const uint8_t* raw = smem + rs * Cfg::RAW_BYTES;
         const uint32_t op = smem_u32(ops + os * Cfg::OP_BYTES);
-        const uint64_t da = make_smem_desc(op + cw * 64 * 128), db = make_smem_desc(op + Cfg::A_BYTES);
-        const uint64_t da_lo = make_smem_desc(op + Cfg::RAW_BYTES + cw * 64 * 128), db_lo = make_smem_desc(op + Cfg::RAW_BYTES + Cfg::A_BYTES);
-        fence_acc(acc);
-        if (!BF16) fence_acc(cor);
-        wgmma_fence();
+        const uint64_t db = make_smem_desc(op), db_lo = make_smem_desc(op + Cfg::B_BYTES);
 #pragma unroll
-        for (int kk = 0; kk < BK / WG_K; ++kk) {
-          // advancing along k inside the 128-byte swizzle row: the descriptors differ only in the start address (units of 16 bytes)
-          const uint64_t ko = (uint64_t)((kk * WG_K * 4) >> 4);
-          const uint32_t accum = (kb | kk) != 0 ? 1u : 0u;
-          if (!BF16) {
-            wgmma_tf32_m64n128k8(cor, da_lo + ko, db + ko, accum);  // lo * hi   } small terms, own accumulator
-            wgmma_tf32_m64n128k8(cor, da + ko, db_lo + ko, 1u);     // hi * lo   }
+        for (int h = 0; h < 2; ++h) {
+          load_a_frags<A_KMAJ, BF16>(raw, r0, lane, h, ah[h], al[h]);
+          if (h == 1) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&raw_empty[rs]);  // this warp holds all of the k-block's A
           }
-          wgmma_tf32_m64n128k8(acc, da + ko, db + ko, accum);       // hi * hi  (bf16-valued operands: the whole product)
+          fence_frags(ah[h]);
+          if (!BF16) fence_frags(al[h]);
+          wgmma_fence();  // orders the A-fragment register writes before the wgmmas that read them
+#pragma unroll
+          for (int q = 0; q < 2; ++q) {
+            const int kk = 2 * h + q;
+            // advancing along k inside the 128-byte swizzle row: the descriptors differ only in the start address (units of 16 bytes)
+            const uint64_t ko = (uint64_t)((kk * WG_K * 4) >> 4);
+            const uint32_t accum = (kb | kk) != 0 ? 1u : 0u;
+            if (!BF16) {
+              wgmma_tf32_m64n128k8(cor, al[h][q], db + ko, accum);  // lo * hi   } small terms, own accumulator
+              wgmma_tf32_m64n128k8(cor, ah[h][q], db_lo + ko, 1u);  // hi * lo   }
+            }
+            wgmma_tf32_m64n128k8(acc, ah[h][q], db + ko, accum);    // hi * hi  (bf16-valued operands: the whole product)
+          }
+          wgmma_commit();
+          // the previous half has retired: its A registers may be rewritten, and after the first half the previous k-block's operand
+          // slot is free
+          wgmma_wait_1();
+          if (h == 0 && kb > 0 && lane == 0) mbar_arrive(&op_empty[os == 0 ? OP_STAGES - 1 : os - 1]);
         }
-        wgmma_commit();
-        wgmma_wait_all();
-        fence_acc(acc);
-        if (!BF16) fence_acc(cor);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&op_empty[os]);
+        if (++rs == RAW_STAGES) { rs = 0; rph ^= 1; }
         if (++os == OP_STAGES) { os = 0; oph ^= 1; }
       }
+      if (nkb > 0) {
+        wgmma_wait_all();
+        if (lane == 0) mbar_arrive(&op_empty[os == 0 ? OP_STAGES - 1 : os - 1]);
+      }
+      fence_acc(acc);
+      if (!BF16) fence_acc(cor);
 
       // ---- epilogue.  Accumulator layout of wgmma m64nN f32: register j of lane l in warp w (of the warpgroup) holds row
       // 16 w + l / 4 + 8 ((j >> 1) & 1), column 8 (j >> 2) + 2 (l & 3) + (j & 1).
-      const int r_base = m0 + cw * 64 + (warp & 3) * 16 + (lane >> 2);
+      const int r_base = m0 + r0;
       const int c_base = n0 + 2 * (lane & 3);
       float* cbase = p.C + p.c_batch_off * zb + p.c_split_off * zs;
       float* ebase = p.extra_col != nullptr ? p.extra_col + p.extra_batch_off * zb + p.extra_split_off * zs : nullptr;
