@@ -139,6 +139,9 @@ class PpoKernels:
         return a
 
     def debug_gemm(self, engine, layout, epilogue, A, B, C, M, N, K, bias=None, aux=None):
+        """One GEMM through the SIMT (engine 0) or wgmma (engine 1) engine; row pitches are taken from the tensors' strides.  Epilogues:
+        0 none, 1 bias+tanh, 3 bias+relu, 5 bias (layout 0); 2 tanh', 4 relu' (layout 1, aux [M, N]); 6 (layout 2, engine 1) rows 0..M-2
+        stored transposed into C[:N], row M-1 into C[N]."""
         nt.check(self.lib.rlx_debug_gemm_f32(int(engine), int(layout), int(epilogue), M, N, K, _f32(A, "A"), A.stride(0), _f32(B, "B"), B.stride(0),
                                              _f32(C, "C"), C.stride(0), _f32(bias, "bias"), _f32(aux, "aux"), aux.stride(0) if aux is not None else 0,
                                              _stream()), "rlx_debug_gemm_f32")

@@ -152,7 +152,7 @@ namespace rlx {
 template <bool A_KMAJ, bool B_KMAJ, int EPI>
 static int aux_gemm(const GemmP& p, int batch, cudaStream_t st, int kclass, long long a_rows, long long b_rows) {
   if (g_aux_gemm_engine == 1 && p.M >= 64 && p.N >= 64 && p.K >= 32 && p.rowsum == nullptr) {
-    const int rc = tc_gemm(p, A_KMAJ, B_KMAJ, tc_epi_of<EPI>(), batch, kclass, a_rows, b_rows, 0, nullptr, 0, 0, st);
+    const int rc = tc_gemm(p, A_KMAJ, B_KMAJ, tc_epi_of<EPI>(), batch, kclass, a_rows, b_rows, st);
     if (rc == RLX_OK) g_aux_tc_gemms.fetch_add(1, std::memory_order_relaxed);   // rlx_aux_tc_gemm_count(): evidence of which engine ran
     if (rc != RLX_ERR_UNSUPPORTED) return rc;
   }

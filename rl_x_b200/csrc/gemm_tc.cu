@@ -129,9 +129,86 @@ __device__ __forceinline__ void load_a_frags(const uint8_t* raw, int r0, int lan
     }
 }
 
+// ---- epilogue.  Accumulator layout of wgmma m64nN f32: register j of lane l in warp w (of the warpgroup) holds row
+// 16 w + l / 4 + 8 ((j >> 1) & 1), column 8 (j >> 2) + 2 (l & 3) + (j & 1).  So a thread owns two rows (row half h = (j >> 1) & 1) and in
+// each the 16 column pairs c = j >> 2; registers 4 c + 2 h and 4 c + 2 h + 1 are the adjacent columns of one pair.
+
+// Epilogue operands (bias, or aux of one row) of a thread's column pairs c0 .. c0 + 7: v[2 c + e] = src[8 c + e].  FULL: the tile lies inside
+// the matrix.  Otherwise a column past the last valid one (offset lim) is not loaded: predicated loads, no branch, and the values of those
+// columns are never stored.
+template <bool FULL>
+__device__ __forceinline__ void load_cols(float (&v)[32], const float* src, int lim, int c0) {
+#pragma unroll
+  for (int i = 2 * c0; i < 2 * c0 + 16; ++i) {
+    const int o = 8 * (i >> 1) + (i & 1);
+    v[i] = (FULL || o <= lim) ? src[o] : 0.f;
+  }
+}
+
+template <int EPI, bool BF16>
+__device__ __forceinline__ float epilogue_op(float x, float e) {
+  if (EPI == TC_EPI_DTANH || EPI == TC_EPI_DRELU)
+    // bf16 mode: linear-backward output rounded to bf16, then tanh_backward rounded to bf16
+    x = (EPI == TC_EPI_DTANH) ? bf16r_if(bf16r_if(x, BF16) * (1.f - e * e), BF16) : ((e > 0.f) ? x : 0.f);
+  if (EPI == TC_EPI_BIAS_TANH || EPI == TC_EPI_BIAS_RELU || EPI == TC_EPI_BIAS) {
+    const float z = (EPI == TC_EPI_BIAS_RELU) ? x + e : bf16r_if(x + e, BF16);  // bf16 mode: Linear output is a bf16 tensor
+    x = (EPI == TC_EPI_BIAS_TANH) ? bf16r_if(tanh_fast(z), BF16) : ((EPI == TC_EPI_BIAS_RELU) ? fmaxf(z, 0.f) : z);
+  }
+  return x;
+}
+
+// acc, cor: main and correction accumulators (the accumulator registers are only read here: a write to them would make ptxas serialise
+// the next tile's wgmmas).  e[h]: the epilogue operand of row half h (the same bias for both); with aux, the thread's 64 values go in four
+// chunks of 8 column pairs, and load_aux(q) issues chunk q + 1 before chunk q is used (chunk 0 is loaded before the MMAs drain): the
+// consumers have no register room for more.  m: global row of row half 0; ct: global column of pair 0.  FULL: every element of the tile
+// is stored, so no bounds tests.
+template <int EPI, bool BF16, bool TRANS, bool FULL, class LoadAux>
+__device__ __forceinline__ void store_tile(const float (&acc)[64], const float (&cor)[64], float (&e)[2][32], const TcParams& p, float* cbase,
+                                           float* ebase, int m, int ct, LoadAux load_aux) {
+  auto x = [&](int j) { return BF16 ? acc[j] : acc[j] + cor[j]; };  // main + correction (fp32 RN)
+  constexpr bool HAS_AUX = (EPI == TC_EPI_DTANH || EPI == TC_EPI_DRELU);
+  if (!TRANS) {
+    // one 8-byte store per column pair: a warp instruction writes 8 whole 32-byte sectors
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int mh = m + 8 * h;
+      float* row = cbase + (long long)mh * p.ldc + ct;
+      const bool row_ok = FULL || mh < p.M;
+#pragma unroll
+      for (int c = 0; c < 16; ++c) {
+        if (HAS_AUX && c % 8 == 0 && 2 * h + c / 8 < 3) load_aux(2 * h + c / 8 + 1);
+        const int j = 4 * c + 2 * h;
+        const float x0 = epilogue_op<EPI, BF16>(x(j), e[HAS_AUX ? h : 0][2 * c]);
+        const float x1 = epilogue_op<EPI, BF16>(x(j + 1), e[HAS_AUX ? h : 0][2 * c + 1]);
+        const int n = ct + 8 * c;
+        if (FULL || (row_ok && n + 1 < p.N)) *reinterpret_cast<float2*>(row + 8 * c) = make_float2(x0, x1);
+        else if (row_ok && n < p.N) row[8 * c] = x0;
+      }
+    }
+  } else {
+    // C^T: element (m, n) at C[n * ldc + m]; scalar stores, each warp instruction fills 4 sectors (8 rows of 4 consecutive m)
+    float* col = cbase + (long long)ct * p.ldc + m;
+    const int ldc = (int)p.ldc;
+#pragma unroll
+    for (int c = 0; c < 16; ++c)
+#pragma unroll
+      for (int q = 0; q < 2; ++q) {
+        const int off = (8 * c + q) * ldc;
+        const int n = ct + 8 * c + q;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float v = x(4 * c + 2 * h + q);
+          const int mh = m + 8 * h;
+          if (FULL || (n < p.N && mh < p.m_main)) col[off + 8 * h] = v;
+          else if (n < p.N && mh == p.m_main && mh < p.M && ebase != nullptr) ebase[n] = v;
+        }
+      }
+  }
+}
+
 // BF16: the bf16-autocast variant (single-pass MMAs on bf16-valued operands, bf16 roundings in the epilogue), a compile-time switch so that
-// the fp32-equivalent kernels carry none of it
-template <bool A_KMAJ, bool B_KMAJ, int EPI, bool BF16>
+// the fp32-equivalent kernels carry none of it.  TRANS: store C^T (the transposed dW1 | db1 GEMM), an instance of its own.
+template <bool A_KMAJ, bool B_KMAJ, int EPI, bool BF16, bool TRANS>
 __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
                                                                  const __grid_constant__ CUtensorMap tmap_b, const TcParams p) {
   constexpr int RAW_STAGES = Cfg::RAW_STAGES, OP_STAGES = Cfg::OP_STAGES;
@@ -292,52 +369,47 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
         if (++rs == RAW_STAGES) { rs = 0; rph ^= 1; }
         if (++os == OP_STAGES) { os = 0; oph ^= 1; }
       }
+
+      // ---- epilogue (layout above).  Its first operands (the bias, or the first aux chunk) are loaded while the last half k-block's MMAs
+      // run, into registers the retired half's A fragments left free.
+      constexpr bool HAS_AUX = (EPI == TC_EPI_DTANH || EPI == TC_EPI_DRELU);
+      constexpr bool HAS_BIAS = (EPI == TC_EPI_BIAS_TANH || EPI == TC_EPI_BIAS_RELU || EPI == TC_EPI_BIAS);
+      const int m = m0 + r0, ct = n0 + 2 * (lane & 3);
+      const bool full = m0 + BM <= (TRANS ? p.m_main : p.M) && n0 + BN <= p.N;  // one test per tile
+      const int clim = p.N - 1 - ct;
+      const float* abase = HAS_AUX ? p.aux + p.aux_batch_off * zb + ct : nullptr;
+      float e[2][32];
+      // aux chunk q: row half q / 2, column pairs 8 (q % 2) .. + 7
+      auto load_aux = [&](int q) {
+        const float* arow = abase + (long long)min(m + 8 * (q >> 1), p.M - 1) * p.ldaux;
+        if (full) load_cols<true>(e[q >> 1], arow, clim, 8 * (q & 1));
+        else load_cols<false>(e[q >> 1], arow, clim, 8 * (q & 1));
+      };
+      if (HAS_BIAS) {
+        const float* b = p.bias + p.bias_batch_off * zb + ct;
+#pragma unroll
+        for (int c0 = 0; c0 < 16; c0 += 8) {
+          if (full) load_cols<true>(e[0], b, clim, c0);
+          else load_cols<false>(e[0], b, clim, c0);
+        }
+      }
+      if (HAS_AUX) load_aux(0);
       if (nkb > 0) {
         wgmma_wait_all();
         if (lane == 0) mbar_arrive(&op_empty[os == 0 ? OP_STAGES - 1 : os - 1]);
       }
       fence_acc(acc);
       if (!BF16) fence_acc(cor);
-
-      // ---- epilogue.  Accumulator layout of wgmma m64nN f32: register j of lane l in warp w (of the warpgroup) holds row
-      // 16 w + l / 4 + 8 ((j >> 1) & 1), column 8 (j >> 2) + 2 (l & 3) + (j & 1).
-      const int r_base = m0 + r0;
-      const int c_base = n0 + 2 * (lane & 3);
       float* cbase = p.C + p.c_batch_off * zb + p.c_split_off * zs;
-      float* ebase = p.extra_col != nullptr ? p.extra_col + p.extra_batch_off * zb + p.extra_split_off * zs : nullptr;
-      constexpr bool HAS_AUX = (EPI == TC_EPI_DTANH || EPI == TC_EPI_DRELU);
-      constexpr bool HAS_BIAS = (EPI == TC_EPI_BIAS_TANH || EPI == TC_EPI_BIAS_RELU || EPI == TC_EPI_BIAS);
-      const float* abase = HAS_AUX ? (p.aux + p.aux_batch_off * zb) : nullptr;
-      const float* bias = HAS_BIAS ? (p.bias + p.bias_batch_off * zb) : nullptr;
-#pragma unroll
-      for (int j = 0; j < 64; ++j) {
-        const int m = r_base + 8 * ((j >> 1) & 1);
-        const int n = c_base + 8 * (j >> 2) + (j & 1);
-        if (m >= p.M || n >= p.N) continue;
-        float x = BF16 ? acc[j] : acc[j] + cor[j];  // main + correction (fp32 RN)
-        if (p.transpose_out) {
-          if (m < p.m_main) cbase[(long long)n * p.ldc + m] = x;
-          else if (m == p.m_main && ebase != nullptr) ebase[n] = x;
-          continue;
-        }
-        if (HAS_AUX) {
-          const float h = abase[(long long)m * p.ldaux + n];
-          // bf16 mode: linear-backward output rounded to bf16, then tanh_backward rounded to bf16
-          x = (EPI == TC_EPI_DTANH) ? bf16r_if(bf16r_if(x, BF16) * (1.f - h * h), BF16) : ((h > 0.f) ? x : 0.f);
-        }
-        if (HAS_BIAS) {
-          const float z = (EPI == TC_EPI_BIAS_RELU) ? x + bias[n] : bf16r_if(x + bias[n], BF16);  // bf16 mode: Linear output is a bf16 tensor
-          x = (EPI == TC_EPI_BIAS_TANH) ? bf16r_if(tanh_fast(z), BF16) : ((EPI == TC_EPI_BIAS_RELU) ? fmaxf(z, 0.f) : z);
-        }
-        if (n < p.n_main) cbase[(long long)m * p.ldc + n] = x;
-        else if (n == p.n_main && ebase != nullptr) ebase[m] = x;
-      }
+      float* ebase = (TRANS && p.extra_row != nullptr) ? p.extra_row + p.extra_batch_off * zb + p.extra_split_off * zs : nullptr;
+      if (full) store_tile<EPI, BF16, TRANS, true>(acc, cor, e, p, cbase, ebase, m, ct, load_aux);
+      else store_tile<EPI, BF16, TRANS, false>(acc, cor, e, p, cbase, ebase, m, ct, load_aux);
     }
   }
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-template <bool A_KMAJ, bool B_KMAJ, int EPI, bool BF16 = false>
+template <bool A_KMAJ, bool B_KMAJ, int EPI, bool BF16 = false, bool TRANS = false>
 static int launch_cfg(const TcOperand& A, const TcOperand& B, TcParams p, int kclass, cudaStream_t stream) {
   CUtensorMap ta, tb;
   int rc = make_tmap(&ta, A.base, A.rows, A.cols, A.ld, 32, A_KMAJ ? BM : BK);
@@ -348,7 +420,8 @@ static int launch_cfg(const TcOperand& A, const TcOperand& B, TcParams p, int kc
   p.tiles_n = (int)ceil_div(p.N, BN);
   const long long tiles = (long long)p.tiles_m * p.tiles_n * p.batch * p.splits;
   if (tiles <= 0) return RLX_OK;
-  auto kern = tc_gemm_kernel<A_KMAJ, B_KMAJ, EPI, BF16>;
+  static_assert(!TRANS || EPI == TC_EPI_NONE, "the transposed store has no epilogue function");
+  auto kern = tc_gemm_kernel<A_KMAJ, B_KMAJ, EPI, BF16, TRANS>;
   static bool attr_done = false;
   if (!attr_done) {
     RLX_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -373,17 +446,14 @@ int tc_supported(const rlx_ppo_dims& d) {
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 // Generic front end over the SIMT engine's GemmP (same meaning of every field).  Supported: all strides multiples of 4 floats,
-// 16-byte aligned bases, batch strides that are pure row or column offsets of the operand tensors.
-int tc_gemm(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int kclass, long long a_rows, long long b_rows, int n_main,
-            float* extra_col, long long extra_batch_off, long long extra_split_off, cudaStream_t stream) {
-  return tc_gemm_t(g, a_kmaj, b_kmaj, epi, batch, kclass, a_rows, b_rows, n_main, extra_col, extra_batch_off, extra_split_off, stream, 0, 0);
-}
-
-int tc_gemm_t(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int kclass, long long a_rows, long long b_rows, int n_main,
-              float* extra_col, long long extra_batch_off, long long extra_split_off, cudaStream_t stream, int transpose_out, int m_main) {
+// 16-byte aligned bases, batch strides that are pure row or column offsets of the operand tensors, and (for the pairwise stores of C) even
+// batch and split offsets of C.  trans: the transposed store (tc_gemm_t).
+static int tc_gemm_impl(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int kclass, long long a_rows, long long b_rows, bool trans,
+                        int m_main, float* extra_row, long long extra_batch_off, long long extra_split_off, cudaStream_t stream) {
   if (g.M <= 0 || g.N <= 0) return RLX_OK;
   if (!aligned16(g.A) || !aligned16(g.B) || !aligned16(g.C) || g.lda % 4 || g.ldb % 4 || g.ldc % 4) return RLX_ERR_UNSUPPORTED;
   if (g.splits > 1 && g.kchunk % BK) return RLX_ERR_UNSUPPORTED;
+  if (!trans && (((batch > 1 ? g.sC : 0) | (g.splits > 1 ? g.sSplitC : 0)) & 1)) return RLX_ERR_UNSUPPORTED;
   if (batch > 1) {
     // A batch stride must be a pure row offset or a pure column offset of the operand's 2-D tensor to become a TMA coordinate.
     // Otherwise (e.g. parameter blocks of different nets that are not a whole number of rows apart) run the nets one by one.
@@ -397,8 +467,8 @@ int tc_gemm_t(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int 
         if (g.aux) gb.aux = g.aux + b * g.sAux;
         gb.sA = gb.sB = gb.sC = gb.sBias = gb.sAux = 0;
         const long long ar = a_rows, br = b_kmaj ? (long long)g.N : (long long)g.K;
-        const int rc = tc_gemm_t(gb, a_kmaj, b_kmaj, epi, 1, kclass, ar, br, n_main, extra_col ? extra_col + b * extra_batch_off : nullptr, 0, extra_split_off, stream,
-                                 transpose_out, m_main);
+        const int rc = tc_gemm_impl(gb, a_kmaj, b_kmaj, epi, 1, kclass, ar, br, trans, m_main, extra_row ? extra_row + b * extra_batch_off : nullptr, 0,
+                                    extra_split_off, stream);
         if (rc) return rc;
       }
       return RLX_OK;
@@ -416,10 +486,8 @@ int tc_gemm_t(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int 
   split_off(g.sA, g.lda, a_kmaj, p.a_mn_off, p.a_k_off);
   split_off(g.sB, g.ldb, b_kmaj, p.b_mn_off, p.b_k_off);
   p.C = g.C; p.ldc = g.ldc; p.c_batch_off = g.sC; p.c_split_off = g.sSplitC;
-  p.n_main = n_main > 0 ? n_main : g.N;
-  p.transpose_out = transpose_out;
-  p.m_main = (transpose_out && m_main > 0) ? m_main : g.M;
-  p.extra_col = extra_col; p.extra_batch_off = extra_batch_off; p.extra_split_off = extra_split_off;
+  p.m_main = (trans && m_main > 0) ? m_main : g.M;
+  p.extra_row = extra_row; p.extra_batch_off = extra_batch_off; p.extra_split_off = extra_split_off;
   p.bias = g.bias; p.bias_batch_off = g.sBias;
   p.aux = g.aux; p.ldaux = g.ldaux; p.aux_batch_off = g.sAux;
   p.single = g.bf16 ? 1 : 0;
@@ -430,6 +498,12 @@ int tc_gemm_t(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int 
               a_kmaj ? (long long)(p.a_k_off * (batch - 1) + g.K) : (long long)(p.a_mn_off * (batch - 1) + g.M), g.lda};
   TcOperand B{g.B, (b_kmaj ? (long long)p.b_mn_off : (long long)p.b_k_off) * (batch - 1) + b_rows,
               b_kmaj ? (long long)(p.b_k_off * (batch - 1) + g.K) : (long long)(p.b_mn_off * (batch - 1) + g.N), g.ldb};
+  if (trans) {
+    if (!a_kmaj && !b_kmaj && epi == TC_EPI_NONE)
+      return p.bf16 ? launch_cfg<false, false, TC_EPI_NONE, true, true>(A, B, p, kclass, stream)
+                    : launch_cfg<false, false, TC_EPI_NONE, false, true>(A, B, p, kclass, stream);
+    return RLX_ERR_UNSUPPORTED;
+  }
   if (p.bf16 && a_kmaj && b_kmaj && epi == TC_EPI_BIAS_TANH) return launch_cfg<true, true, TC_EPI_BIAS_TANH, true>(A, B, p, kclass, stream);
   if (p.bf16 && a_kmaj && !b_kmaj && epi == TC_EPI_DTANH) return launch_cfg<true, false, TC_EPI_DTANH, true>(A, B, p, kclass, stream);
   if (p.bf16 && !a_kmaj && !b_kmaj && epi == TC_EPI_NONE) return launch_cfg<false, false, TC_EPI_NONE, true>(A, B, p, kclass, stream);
@@ -443,6 +517,15 @@ int tc_gemm_t(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int 
   if (a_kmaj && !b_kmaj && epi == TC_EPI_NONE) return launch_cfg<true, false, TC_EPI_NONE>(A, B, p, kclass, stream);
   if (!a_kmaj && !b_kmaj && epi == TC_EPI_NONE) return launch_cfg<false, false, TC_EPI_NONE>(A, B, p, kclass, stream);
   return RLX_ERR_UNSUPPORTED;
+}
+
+int tc_gemm(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int kclass, long long a_rows, long long b_rows, cudaStream_t stream) {
+  return tc_gemm_impl(g, a_kmaj, b_kmaj, epi, batch, kclass, a_rows, b_rows, false, 0, nullptr, 0, 0, stream);
+}
+
+int tc_gemm_t(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int kclass, long long a_rows, long long b_rows, int m_main, float* extra_row,
+              long long extra_batch_off, long long extra_split_off, cudaStream_t stream) {
+  return tc_gemm_impl(g, a_kmaj, b_kmaj, epi, batch, kclass, a_rows, b_rows, true, m_main, extra_row, extra_batch_off, extra_split_off, stream);
 }
 
 }  // namespace rlx

@@ -25,10 +25,9 @@ struct TcParams {
   int a_mn_off, a_k_off, b_mn_off, b_k_off;
   float* C;
   long long ldc, c_batch_off, c_split_off;
-  int n_main;                // columns >= n_main are not stored to C; column == n_main goes to extra_col (bias-gradient trick)
-  int transpose_out;         // store C^T: element (m, n) at C[n * ldc + m]; rows >= m_main are not stored, row == m_main goes to extra_col[n]
+  // transposed-store kernels only: element (m, n) at C[n * ldc + m] for m < m_main; row m_main goes to extra_row[n] (bias-gradient trick)
   int m_main;
-  float* extra_col;          // [z][M] or null
+  float* extra_row;          // [z][N] or null
   long long extra_batch_off, extra_split_off;
   const float* bias;         // TC_EPI_BIAS_TANH
   long long bias_batch_off;

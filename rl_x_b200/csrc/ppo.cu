@@ -478,7 +478,7 @@ static int launch_head_wgrad(const PpoLayout& L, const TrainPlan& P, long long m
     g3.sA = 0; g3.sB = H; g3.sC = (long long)dh_ld * H;
     g3.splits = S3.splits; g3.kchunk = S3.kchunk; g3.sSplitC = 2LL * dh_ld * H;
     g3.bf16 = bf16;
-    const int rc = tc_gemm(g3, false, false, TC_NONE, 2, KC_HEAD_WGRAD, m, m, 0, nullptr, 0, 0, st);
+    const int rc = tc_gemm(g3, false, false, TC_NONE, 2, KC_HEAD_WGRAD, m, m, st);
     if (rc == RLX_OK) {
       // net 1 (critic half of H2), row `act` of its [dh_ld, H] block
       w3 = W3Partials{part3, S3.splits, 2LL * dh_ld * H, (long long)dh_ld * H + (long long)A * H};
@@ -544,7 +544,7 @@ static int launch_hidden_backward(const PpoLayout& L, const TrainPlan& P, const 
     gt.M = O + 1; gt.N = 2 * H; gt.K = (int)m;
     gt.lda = (int)ldx; gt.ldb = 2 * H; gt.ldc = O;
     gt.splits = S1.splits; gt.kchunk = S1.kchunk; gt.sSplitC = 2LL * H * O;
-    rc = tc_gemm_t(gt, false, false, TC_NONE, 1, KC_GEMM_DW, m, m, 0, rs1, 0, 2LL * H, st, 1, O);
+    rc = tc_gemm_t(gt, false, false, TC_NONE, 1, KC_GEMM_DW, m, m, O, rs1, 0, 2LL * H, st);
     if (rc == RLX_OK) {
       s1 = S1.splits;
       return RLX_OK;
@@ -765,13 +765,18 @@ extern "C" int rlx_ppo_update_epoch_sharded_f32(const rlx_ppo_minibatch_args* fi
 }
 
 // Test hook: one plain GEMM through either engine (single batch, no split): layout 0 = A k-major, B k-major (C = A B^T);
-// 1 = A k-major, B n-major (C = A B); 2 = A m-major, B n-major (C = A^T B, A is [K, M]).  epilogue 0 none, 1 bias+tanh, 2 tanh'.
+// 1 = A k-major, B n-major (C = A B); 2 = A m-major, B n-major (C = A^T B, A is [K, M]).  Epilogue 0 none, 1 bias+tanh, 3 bias+relu,
+// 5 bias (layout 0), 2 tanh', 4 relu' (layout 1, aux [M, ldaux]); 6 (layout 2, wgmma engine only) the transposed store with an extra row:
+// rows 0 .. M-2 of the product go transposed into C [N, ldc], row M-1 into row N of C.
 extern "C" int rlx_debug_gemm_f32(int engine, int layout, int epilogue, int64_t M, int64_t N, int64_t K, const float* A, int64_t lda,
                                   const float* B, int64_t ldb, float* C, int64_t ldc, const float* bias, const float* aux, int64_t ldaux,
                                   void* stream) {
   RLX_CHECK_ARG(A && B && C && M > 0 && N > 0 && K > 0, "bad arguments");
   RLX_CHECK_ARG(engine == 0 || engine == 1, "unknown engine (0 = SIMT, 1 = wgmma tensor cores)");
-  RLX_CHECK_ARG((epilogue == 0) || (epilogue == 1 && layout == 0 && bias) || (epilogue == 2 && layout == 1 && aux), "unsupported epilogue/layout");
+  const bool bias_epi = epilogue == 1 || epilogue == 3 || epilogue == 5, aux_epi = epilogue == 2 || epilogue == 4;
+  RLX_CHECK_ARG((epilogue == 0) || (bias_epi && layout == 0 && bias) || (aux_epi && layout == 1 && aux) ||
+                    (epilogue == 6 && layout == 2 && engine == 1 && M >= 2),
+                "unsupported epilogue/layout");
   GemmP g{};
   g.A = A; g.B = B; g.C = C; g.bias = bias; g.aux = aux;
   g.M = (int)M; g.N = (int)N; g.K = (int)K;
@@ -781,13 +786,17 @@ extern "C" int rlx_debug_gemm_f32(int engine, int layout, int epilogue, int64_t 
   const bool a_k = layout != 2, b_k = layout == 0;
   const long long a_rows = a_k ? M : K, b_rows = b_k ? N : K;
   if (engine == 1) {
-    const int rc = tc_gemm(g, a_k, b_k, epilogue, 1, KC_OTHER, a_rows, b_rows, 0, nullptr, 0, 0, st);
+    const int rc = epilogue == 6 ? tc_gemm_t(g, a_k, b_k, TC_NONE, 1, KC_OTHER, a_rows, b_rows, (int)M - 1, C + N * ldc, 0, 0, st)
+                                 : tc_gemm(g, a_k, b_k, epilogue, 1, KC_OTHER, a_rows, b_rows, st);
     if (rc == RLX_ERR_UNSUPPORTED) set_error("rlx_debug_gemm_f32: shape/alignment not supported by the wgmma engine");
     return rc;
   }
   if (layout == 0 && epilogue == 1) return launch_sgemm<true, true, EPI_BIAS_TANH>(g, 1, st);
+  if (layout == 0 && epilogue == 3) return launch_sgemm<true, true, EPI_BIAS_RELU>(g, 1, st);
+  if (layout == 0 && epilogue == 5) return launch_sgemm<true, true, EPI_BIAS>(g, 1, st);
   if (layout == 0) return launch_sgemm<true, true, EPI_NONE>(g, 1, st);
   if (layout == 1 && epilogue == 2) return launch_sgemm<true, false, EPI_DTANH>(g, 1, st);
+  if (layout == 1 && epilogue == 4) return launch_sgemm<true, false, EPI_DRELU>(g, 1, st);
   if (layout == 1) return launch_sgemm<true, false, EPI_NONE>(g, 1, st);
   return launch_sgemm<false, false, EPI_NONE>(g, 1, st);
 }
