@@ -58,10 +58,15 @@ int rlx_set_aux_gemm_engine(int engine);
 uint64_t rlx_aux_tc_gemm_count(void);     /* GEMMs of those two paths that ran on the wgmma engine since load */
 
 /* Test hook: one plain fp32 GEMM through either engine (0 = SIMT, 1 = wgmma; any other value is RLX_ERR_INVALID_ARG).  layout 0: C[M,N] = A[M,K] B[N,K]^T; 1: C = A[M,K] B[K,N];
- * 2: C = A[K,M]^T B[K,N].  epilogue 0 none, 1 tanh(x + bias[n]) (layout 0), 2 x * (1 - aux[m,n]^2) (layout 1). */
+ * 2: C = A[K,M]^T B[K,N].  epilogue 0 none, 1 tanh(x + bias[n]) (layout 0), 2 x * (1 - aux[m,n]^2) (layout 1).  Layouts 3 / 4 (wgmma engine,
+ * epilogue 1 / 2): layout 0 / 1 with B split into tf32 hi / lo copies first (layout 4: transposed to [N, K]; K a multiple of 4), through
+ * the engine's pre-split instances. */
 int rlx_debug_gemm_f32(int engine, int layout, int epilogue, int64_t M, int64_t N, int64_t K, const float* A, int64_t lda,
                        const float* B, int64_t ldb, float* C, int64_t ldc, const float* bias, const float* aux, int64_t ldaux,
                        void* stream);
+/* Test hook: tf32 hi / lo split of src [batch][rows][cols]: hi = bits & 0xFFFFE000, lo = src - hi, into hi / lo of the same layout, or with
+ * trans != 0 of layout [batch][cols][rows].  The minibatch update splits its weights this way for the wgmma engine. */
+int rlx_debug_tf32_split_f32(const float* src, int64_t batch, int64_t rows, int64_t cols, int trans, float* hi, float* lo, void* stream);
 
 /* ------------------------------------------------------------------------------- numpy-compatible host RNG -- */
 /* ref: self.rng = np.random.default_rng(self.seed)  (ppo.py:72; sac.py replay_buffer.py:8) — Generator(PCG64(SeedSequence(seed))).

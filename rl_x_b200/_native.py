@@ -231,6 +231,7 @@ _SIGNATURES = {
     "rlx_gather_minibatch_f32": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64] + [C.c_void_p] * 10 + [C.c_int64, C.c_void_p]),
     "rlx_debug_gemm_f32": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
                                      C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "rlx_debug_tf32_split_f32": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rlx_advantage_stats_f32": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
     "rlx_segment_moments_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rlx_ppo_minibatch_workspace_bytes": (C.c_size_t, [C.POINTER(PpoDims), C.c_int64]),

@@ -141,10 +141,19 @@ class PpoKernels:
     def debug_gemm(self, engine, layout, epilogue, A, B, C, M, N, K, bias=None, aux=None):
         """One GEMM through the SIMT (engine 0) or wgmma (engine 1) engine; row pitches are taken from the tensors' strides.  Epilogues:
         0 none, 1 bias+tanh, 3 bias+relu, 5 bias (layout 0); 2 tanh', 4 relu' (layout 1, aux [M, N]); 6 (layout 2, engine 1) rows 0..M-2
-        stored transposed into C[:N], row M-1 into C[N]."""
+        stored transposed into C[:N], row M-1 into C[N].  Layouts 3 / 4 (engine 1, epilogue 1 / 2): layout 0 / 1 with B split into tf32
+        hi / lo copies first (layout 4 transposes it; K a multiple of 4), through the engine's pre-split instances."""
         nt.check(self.lib.rlx_debug_gemm_f32(int(engine), int(layout), int(epilogue), M, N, K, _f32(A, "A"), A.stride(0), _f32(B, "B"), B.stride(0),
                                              _f32(C, "C"), C.stride(0), _f32(bias, "bias"), _f32(aux, "aux"), aux.stride(0) if aux is not None else 0,
                                              _stream()), "rlx_debug_gemm_f32")
+
+    def debug_tf32_split(self, src, trans, hi, lo):
+        """tf32 hi / lo split of a contiguous [batch, rows, cols] tensor, the one the minibatch update makes of its weights: hi / lo
+        [batch, rows, cols], or [batch, cols, rows] with trans."""
+        assert src.dim() == 3 and src.is_contiguous() and hi.is_contiguous() and lo.is_contiguous()
+        b, r, c = src.shape
+        nt.check(self.lib.rlx_debug_tf32_split_f32(_f32(src, "src"), b, r, c, int(bool(trans)), _f32(hi, "hi"), _f32(lo, "lo"), _stream()),
+                 "rlx_debug_tf32_split_f32")
 
     def states_pitch(self):
         """Row pitch (floats) of the gathered-states buffer: obs_dim plus a constant-one column, rounded up to 16 bytes."""

@@ -13,6 +13,17 @@ int tc_gemm_t(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int 
               long long extra_batch_off, long long extra_split_off, cudaStream_t stream);
 enum { TC_NONE = 0, TC_BIAS_TANH = 1, TC_DTANH = 2, TC_BIAS_RELU = 3, TC_DRELU = 4, TC_BIAS = 5 };
 
+// tf32 hi / lo split of fp32 matrices for GemmP::b_hi / b_lo, the wgmma engine's converter arithmetic: hi = x & 0xFFFFE000, lo = x - hi.
+// src is [batch][rows][cols] contiguous; hi / lo get the same layout, or with trans [batch][cols][rows].  One launch for all jobs.
+struct Tf32SplitJob {
+  const float* src;
+  float* hi;
+  float* lo;
+  int batch, rows, cols, trans;
+};
+constexpr int kMaxTf32SplitJobs = 3;
+int tf32_split(const Tf32SplitJob* jobs, int njobs, int kclass, cudaStream_t stream);
+
 template <int EPI>
 constexpr int tc_epi_of() {
   return EPI == EPI_BIAS_TANH ? TC_BIAS_TANH : EPI == EPI_DTANH ? TC_DTANH : EPI == EPI_BIAS_RELU ? TC_BIAS_RELU : EPI == EPI_DRELU ? TC_DRELU

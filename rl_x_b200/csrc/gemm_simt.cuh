@@ -27,6 +27,8 @@ struct GemmP {
   int bf16;           // bf16-autocast mode: operands are bf16 values; Linear outputs / activations / their gradients are rounded to bf16
                       // where torch's autocast rounds them (EPI_NONE outputs - split-K partials of weight gradients - stay fp32: they
                       // are rounded once after the full reduction)
+  const float* b_hi;  // optional, wgmma engine only: tf32 hi / lo copies of B (tf32_split), K-major [N, K] with pitch ldb and batch stride sB;
+  const float* b_lo;  // the forward (bias+tanh) and dX (tanh') GEMMs then skip the B converter.  The SIMT engine reads B.
 };
 
 constexpr int GBM = 128, GBN = 128, GBK = 8, GPAD = 4;

@@ -17,6 +17,9 @@
 //                 relu / plain, stores to C (or C^T)
 // A raw slot is refilled once the converter has used its B and all 8 consumer warps hold its A in registers; an operand slot once the
 // wgmmas that read it have retired.
+// Pre-split instances (SPLIT_B: B is a weight matrix whose tf32 hi / lo copies tf32_split made in global memory, K-major): thread 0
+// TMA-loads A, hi B and lo B into one stage [A | hi B | lo B] of a 4-stage ring, which is exactly the layout the converter would have
+// written; warpgroup 0 does no conversion, and a stage is refilled once the wgmmas that read it have retired.
 // Operand layouts in global memory: K-major (row = m or n, 32 consecutive k = one 128-byte swizzle row) or MN-major (row = k, 32
 // consecutive m/n per 128-byte row; used by the weight-gradient GEMMs whose reduction runs over the minibatch rows).  The converter
 // transposes MN-major B tiles to K-major; the consumers' fragment reads transpose MN-major A.  Out-of-bounds parts of a box are
@@ -37,10 +40,14 @@ struct Cfg {
   // the consumers hold up to two operand slots (the k-block being issued and the one retiring), so 4 stages let the converter run two ahead
   static constexpr int RAW_STAGES = 3, OP_STAGES = 4;
   static constexpr int SMEM_BYTES = RAW_STAGES * RAW_BYTES + OP_STAGES * OP_BYTES + 1024 /*barriers*/ + 1024 /*alignment slack*/;
+  // pre-split B: stage [A | hi B | lo B]; the consumers hold up to two stages, so 4 stages let the TMA run two ahead
+  static constexpr int SPLIT_STAGE_BYTES = A_BYTES + 2 * B_BYTES;  // 48 KB
+  static constexpr int SPLIT_STAGES = 4;
+  static constexpr int SPLIT_SMEM_BYTES = SPLIT_STAGES * SPLIT_STAGE_BYTES + 1024 + 1024;
   // consumers: 2 x 64 accumulators + 2 half k-blocks x 16 A-fragment registers
   static constexpr int PRODUCER_REGS = 56, CONSUMER_REGS = 224;
 };
-static_assert(Cfg::SMEM_BYTES <= 227 * 1024, "shared memory of one H100 block");
+static_assert(Cfg::SMEM_BYTES <= 227 * 1024 && Cfg::SPLIT_SMEM_BYTES <= 227 * 1024, "shared memory of one H100 block");
 static_assert(Cfg::PRODUCER_REGS * 128 + Cfg::CONSUMER_REGS * 256 <= 65536, "register file of one SM");
 
 // One B tile (ROWS x BK) from its raw stage to K-major swizzled hi / lo tiles.  In the 128-byte swizzle every 16-byte chunk
@@ -207,17 +214,21 @@ __device__ __forceinline__ void store_tile(const float (&acc)[64], const float (
 }
 
 // BF16: the bf16-autocast variant (single-pass MMAs on bf16-valued operands, bf16 roundings in the epilogue), a compile-time switch so that
-// the fp32-equivalent kernels carry none of it.  TRANS: store C^T (the transposed dW1 | db1 GEMM), an instance of its own.
-template <bool A_KMAJ, bool B_KMAJ, int EPI, bool BF16, bool TRANS>
-__global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
-                                                                 const __grid_constant__ CUtensorMap tmap_b, const TcParams p) {
-  constexpr int RAW_STAGES = Cfg::RAW_STAGES, OP_STAGES = Cfg::OP_STAGES;
+// the fp32-equivalent kernels carry none of it.  TRANS: store C^T (the transposed dW1 | db1 GEMM), an instance of its own.  SPLIT_B: B
+// arrives pre-split (tmap_b = hi, tmap_b_lo = lo, both K-major); the other instances do not read tmap_b_lo.
+template <bool A_KMAJ, bool B_KMAJ, int EPI, bool BF16, bool TRANS, bool SPLIT_B>
+__global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                                                                 const __grid_constant__ CUtensorMap tmap_b_lo, const TcParams p) {
+  static_assert(!SPLIT_B || (B_KMAJ && !BF16), "pre-split B is K-major fp32 hi / lo");
+  // SPLIT_B: one ring; a raw stage is the whole stage [A | hi B | lo B], raw_full / op_empty are its full / empty barriers (rs == os)
+  constexpr int RAW_STAGES = SPLIT_B ? Cfg::SPLIT_STAGES : Cfg::RAW_STAGES, OP_STAGES = SPLIT_B ? Cfg::SPLIT_STAGES : Cfg::OP_STAGES;
+  constexpr int RAW_BYTES = SPLIT_B ? Cfg::SPLIT_STAGE_BYTES : Cfg::RAW_BYTES;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment (swizzle atoms) as an OFFSET on the __shared__ pointer: a round trip through uintptr_t makes the compiler lose
   // the shared address space and emit generic loads / stores
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* ops = smem + RAW_STAGES * Cfg::RAW_BYTES;
-  uint64_t* raw_full = reinterpret_cast<uint64_t*>(ops + OP_STAGES * Cfg::OP_BYTES);  // [RAW_STAGES]  TMA landed
+  uint8_t* ops = smem + RAW_STAGES * RAW_BYTES;
+  uint64_t* raw_full = reinterpret_cast<uint64_t*>(ops + (SPLIT_B ? 0 : OP_STAGES * Cfg::OP_BYTES));  // [RAW_STAGES]  TMA landed
   uint64_t* raw_empty = raw_full + RAW_STAGES;                                        // [RAW_STAGES]  B converted, A in registers
   uint64_t* op_full = raw_empty + RAW_STAGES;                                         // [OP_STAGES]   hi / lo B tiles written
   uint64_t* op_empty = op_full + OP_STAGES;                                           // [OP_STAGES]   wgmmas of the slot retired
@@ -226,6 +237,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_b);
+    if (SPLIT_B) prefetch_tmap(&tmap_b_lo);
     for (int s = 0; s < RAW_STAGES; ++s) {
       mbar_init(&raw_full[s], 1);
       mbar_init(&raw_empty[s], 1 + 8);  // the converter + one arrival per consumer warp
@@ -257,6 +269,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
     setmaxnreg_dec<Cfg::PRODUCER_REGS>();
     const int t = threadIdx.x;
     // load cursor: the k-blocks of this CTA's tiles in consumption order; a raw slot is refilled once its raw_empty phase completes
+    // (SPLIT_B: once its op_empty phase completes).  Returns false past the last k-block.
+    uint64_t* ld_empty = SPLIT_B ? op_empty : raw_empty;
     int ld_tile = blockIdx.x, ld_kb = 0, ld_count = 0;
     auto load_next = [&]() {
       while (ld_tile < num_tiles) {
@@ -268,12 +282,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
           continue;
         }
         const int slot = ld_count % RAW_STAGES;
-        mbar_wait(&raw_empty[slot], ((ld_count / RAW_STAGES) & 1) ^ 1);  // the first round passes: a fresh barrier's previous phase
-        uint8_t* sa = smem + slot * Cfg::RAW_BYTES;
+        mbar_wait(&ld_empty[slot], ((ld_count / RAW_STAGES) & 1) ^ 1);  // the first round passes: a fresh barrier's previous phase
+        uint8_t* sa = smem + slot * RAW_BYTES;
         uint8_t* sb = sa + Cfg::A_BYTES;
         uint64_t* bar = &raw_full[slot];
         const int k0 = kbeg + ld_kb * BK;
-        mbar_arrive_expect_tx(bar, Cfg::RAW_BYTES);
+        mbar_arrive_expect_tx(bar, RAW_BYTES);
         if (A_KMAJ) {
           tma_load_2d(&tmap_a, bar, sa, p.a_k_off * zb + k0, p.a_mn_off * zb + m0);
         } else {
@@ -282,15 +296,24 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
         }
         if (B_KMAJ) {
           tma_load_2d(&tmap_b, bar, sb, p.b_k_off * zb + k0, p.b_mn_off * zb + n0);
+          if (SPLIT_B) tma_load_2d(&tmap_b_lo, bar, sb + Cfg::B_BYTES, p.b_k_off * zb + k0, p.b_mn_off * zb + n0);
         } else {
 #pragma unroll
           for (int j = 0; j < BN / 32; ++j) tma_load_2d(&tmap_b, bar, sb + j * (BK * 128), p.b_mn_off * zb + n0 + 32 * j, p.b_k_off * zb + k0);
         }
         ++ld_kb;
         ++ld_count;
-        return;
+        return true;
       }
+      return false;
     };
+    if constexpr (SPLIT_B) {
+      // nothing to convert: thread 0 streams the k-blocks through the ring, the rest of the warpgroup is done
+      if (t == 0)
+        while (load_next()) {
+        }
+      return;
+    }
     if (t == 0)
       for (int i = 0; i < RAW_STAGES; ++i) load_next();
     int rs = 0, os = 0;
@@ -334,14 +357,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
       tile_coords(tile, zb, zs, m0, n0, kbeg, nkb);
       for (int kb = 0; kb < nkb; ++kb) {
         mbar_wait(&raw_full[rs], rph);
-        mbar_wait(&op_full[os], oph);
-        const uint8_t* raw = smem + rs * Cfg::RAW_BYTES;
-        const uint32_t op = smem_u32(ops + os * Cfg::OP_BYTES);
+        if (!SPLIT_B) mbar_wait(&op_full[os], oph);
+        const uint8_t* raw = smem + rs * RAW_BYTES;
+        const uint32_t op = SPLIT_B ? smem_u32(raw + Cfg::A_BYTES) : smem_u32(ops + os * Cfg::OP_BYTES);
         const uint64_t db = make_smem_desc(op), db_lo = make_smem_desc(op + Cfg::B_BYTES);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           load_a_frags<A_KMAJ, BF16>(raw, r0, lane, h, ah[h], al[h]);
-          if (h == 1) {
+          if (!SPLIT_B && h == 1) {
             __syncwarp();
             if (lane == 0) mbar_arrive(&raw_empty[rs]);  // this warp holds all of the k-block's A
           }
@@ -409,28 +432,36 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-template <bool A_KMAJ, bool B_KMAJ, int EPI, bool BF16 = false, bool TRANS = false>
-static int launch_cfg(const TcOperand& A, const TcOperand& B, TcParams p, int kclass, cudaStream_t stream) {
-  CUtensorMap ta, tb;
+// SPLIT_B: B.base is the hi copy, b_lo the lo copy (same extents and pitch)
+template <bool A_KMAJ, bool B_KMAJ, int EPI, bool BF16 = false, bool TRANS = false, bool SPLIT_B = false>
+static int launch_cfg(const TcOperand& A, const TcOperand& B, TcParams p, int kclass, cudaStream_t stream, const float* b_lo = nullptr) {
+  CUtensorMap ta, tb, tb_lo;
   int rc = make_tmap(&ta, A.base, A.rows, A.cols, A.ld, 32, A_KMAJ ? BM : BK);
   if (rc) return rc;
   rc = make_tmap(&tb, B.base, B.rows, B.cols, B.ld, 32, B_KMAJ ? BN : BK);
   if (rc) return rc;
+  if (SPLIT_B) {
+    rc = make_tmap(&tb_lo, b_lo, B.rows, B.cols, B.ld, 32, BN);
+    if (rc) return rc;
+  } else {
+    tb_lo = tb;  // not read
+  }
   p.tiles_m = (int)ceil_div(p.M, BM);
   p.tiles_n = (int)ceil_div(p.N, BN);
   const long long tiles = (long long)p.tiles_m * p.tiles_n * p.batch * p.splits;
   if (tiles <= 0) return RLX_OK;
   static_assert(!TRANS || EPI == TC_EPI_NONE, "the transposed store has no epilogue function");
-  auto kern = tc_gemm_kernel<A_KMAJ, B_KMAJ, EPI, BF16, TRANS>;
+  auto kern = tc_gemm_kernel<A_KMAJ, B_KMAJ, EPI, BF16, TRANS, SPLIT_B>;
+  constexpr int smem = SPLIT_B ? Cfg::SPLIT_SMEM_BYTES : Cfg::SMEM_BYTES;
   static bool attr_done = false;
   if (!attr_done) {
-    RLX_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    RLX_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_done = true;
   }
   const unsigned grid = (unsigned)std::min<long long>(tiles, sm_count());
   const double flops = 2.0 * p.M * p.N * (double)p.K * p.batch;
-  const double bytes = 4.0 * p.batch * ((double)p.M * p.K + (double)p.N * p.K + (double)p.M * p.N * p.splits);
-  RLX_LAUNCH_C(kclass, flops, bytes, kern, grid, NUM_THREADS, Cfg::SMEM_BYTES, stream, ta, tb, p);
+  const double bytes = 4.0 * p.batch * ((double)p.M * p.K + (SPLIT_B ? 2.0 : 1.0) * p.N * p.K + (double)p.M * p.N * p.splits);
+  RLX_LAUNCH_C(kclass, flops, bytes, kern, grid, NUM_THREADS, smem, stream, ta, tb, tb_lo, p);
   return RLX_OK;
 }
 
@@ -451,6 +482,13 @@ static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 static int tc_gemm_impl(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int kclass, long long a_rows, long long b_rows, bool trans,
                         int m_main, float* extra_row, long long extra_batch_off, long long extra_split_off, cudaStream_t stream) {
   if (g.M <= 0 || g.N <= 0) return RLX_OK;
+  // pre-split B (g.b_hi / g.b_lo, K-major [N, K] per batch entry): the instances that exist take it, the rest read g.B through the converter
+  const bool split_b = g.b_hi != nullptr && !g.bf16 && !trans && a_kmaj && (epi == TC_EPI_BIAS_TANH || epi == TC_EPI_DTANH);
+  if (split_b) {
+    if (!aligned16(g.b_hi) || !aligned16(g.b_lo)) return RLX_ERR_UNSUPPORTED;
+    b_kmaj = true;
+    b_rows = g.N;
+  }
   if (!aligned16(g.A) || !aligned16(g.B) || !aligned16(g.C) || g.lda % 4 || g.ldb % 4 || g.ldc % 4) return RLX_ERR_UNSUPPORTED;
   if (g.splits > 1 && g.kchunk % BK) return RLX_ERR_UNSUPPORTED;
   if (!trans && (((batch > 1 ? g.sC : 0) | (g.splits > 1 ? g.sSplitC : 0)) & 1)) return RLX_ERR_UNSUPPORTED;
@@ -463,6 +501,7 @@ static int tc_gemm_impl(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int b
       for (int b = 0; b < batch; ++b) {
         GemmP gb = g;
         gb.A = g.A + b * g.sA; gb.B = g.B + b * g.sB; gb.C = g.C + b * g.sC;
+        if (g.b_hi) { gb.b_hi = g.b_hi + b * g.sB; gb.b_lo = g.b_lo + b * g.sB; }
         if (g.bias) gb.bias = g.bias + b * g.sBias;
         if (g.aux) gb.aux = g.aux + b * g.sAux;
         gb.sA = gb.sB = gb.sC = gb.sBias = gb.sAux = 0;
@@ -496,7 +535,7 @@ static int tc_gemm_impl(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int b
   // (TMA zero-fills beyond them); batch entries that sit at row offsets extend the tensor accordingly.
   TcOperand A{g.A, (a_kmaj ? (long long)p.a_mn_off : (long long)p.a_k_off) * (batch - 1) + a_rows,
               a_kmaj ? (long long)(p.a_k_off * (batch - 1) + g.K) : (long long)(p.a_mn_off * (batch - 1) + g.M), g.lda};
-  TcOperand B{g.B, (b_kmaj ? (long long)p.b_mn_off : (long long)p.b_k_off) * (batch - 1) + b_rows,
+  TcOperand B{split_b ? g.b_hi : g.B, (b_kmaj ? (long long)p.b_mn_off : (long long)p.b_k_off) * (batch - 1) + b_rows,
               b_kmaj ? (long long)(p.b_k_off * (batch - 1) + g.K) : (long long)(p.b_mn_off * (batch - 1) + g.N), g.ldb};
   if (trans) {
     if (!a_kmaj && !b_kmaj && epi == TC_EPI_NONE)
@@ -508,6 +547,8 @@ static int tc_gemm_impl(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int b
   if (p.bf16 && a_kmaj && !b_kmaj && epi == TC_EPI_DTANH) return launch_cfg<true, false, TC_EPI_DTANH, true>(A, B, p, kclass, stream);
   if (p.bf16 && !a_kmaj && !b_kmaj && epi == TC_EPI_NONE) return launch_cfg<false, false, TC_EPI_NONE, true>(A, B, p, kclass, stream);
   if (p.bf16) return RLX_ERR_UNSUPPORTED;
+  if (split_b && epi == TC_EPI_BIAS_TANH) return launch_cfg<true, true, TC_EPI_BIAS_TANH, false, false, true>(A, B, p, kclass, stream, g.b_lo);
+  if (split_b && epi == TC_EPI_DTANH) return launch_cfg<true, true, TC_EPI_DTANH, false, false, true>(A, B, p, kclass, stream, g.b_lo);
   if (a_kmaj && b_kmaj && epi == TC_EPI_BIAS_TANH) return launch_cfg<true, true, TC_EPI_BIAS_TANH>(A, B, p, kclass, stream);
   if (a_kmaj && b_kmaj && epi == TC_EPI_NONE) return launch_cfg<true, true, TC_EPI_NONE>(A, B, p, kclass, stream);
   if (a_kmaj && b_kmaj && epi == TC_EPI_BIAS_RELU) return launch_cfg<true, true, TC_EPI_BIAS_RELU>(A, B, p, kclass, stream);
@@ -526,6 +567,59 @@ int tc_gemm(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int kc
 int tc_gemm_t(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int kclass, long long a_rows, long long b_rows, int m_main, float* extra_row,
               long long extra_batch_off, long long extra_split_off, cudaStream_t stream) {
   return tc_gemm_impl(g, a_kmaj, b_kmaj, epi, batch, kclass, a_rows, b_rows, true, m_main, extra_row, extra_batch_off, extra_split_off, stream);
+}
+
+// ------------------------------------------------------------------------------------------------ tf32 hi / lo split
+namespace tc {
+struct Tf32SplitJobs {
+  Tf32SplitJob job[kMaxTf32SplitJobs];
+  int first_tile[kMaxTf32SplitJobs + 1];  // CTA range of each job
+};
+
+// one 32 x 32 tile of one job per CTA (256 threads), through shared memory so that the transposed writes are coalesced too
+__global__ void __launch_bounds__(256) tf32_split_kernel(const __grid_constant__ Tf32SplitJobs J) {
+  __shared__ float tile[32][33];
+  int j = 0;
+  while ((int)blockIdx.x >= J.first_tile[j + 1]) ++j;
+  const Tf32SplitJob& s = J.job[j];
+  const int tiles_c = (s.cols + 31) / 32, tiles_rc = ((s.rows + 31) / 32) * tiles_c;
+  const int b = (int)blockIdx.x - J.first_tile[j];
+  const int z = b / tiles_rc, r0 = (b % tiles_rc) / tiles_c * 32, c0 = b % tiles_c * 32;
+  const long long zoff = (long long)z * s.rows * s.cols;
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+#pragma unroll
+  for (int i = ty; i < 32; i += 8)
+    if (r0 + i < s.rows && c0 + tx < s.cols) tile[i][tx] = s.src[zoff + (long long)(r0 + i) * s.cols + c0 + tx];
+  __syncthreads();
+#pragma unroll
+  for (int i = ty; i < 32; i += 8) {
+    // destination row / column and source tile element of this thread
+    const int dr = s.trans ? c0 + i : r0 + i, dc = s.trans ? r0 + tx : c0 + tx, dcols = s.trans ? s.rows : s.cols;
+    if (dr < (s.trans ? s.cols : s.rows) && dc < dcols) {
+      const float x = s.trans ? tile[tx][i] : tile[i][tx];
+      const uint32_t h = __float_as_uint(x) & 0xFFFFE000u;  // convert_tile's split
+      const long long o = zoff + (long long)dr * dcols + dc;
+      s.hi[o] = __uint_as_float(h);
+      s.lo[o] = x - __uint_as_float(h);
+    }
+  }
+}
+}  // namespace tc
+
+int tf32_split(const Tf32SplitJob* jobs, int njobs, int kclass, cudaStream_t stream) {
+  if (njobs < 1 || njobs > kMaxTf32SplitJobs) return RLX_ERR_INVALID_ARG;
+  Tf32SplitJobs J{};
+  long long tiles = 0, elems = 0;
+  for (int i = 0; i < njobs; ++i) {
+    J.job[i] = jobs[i];
+    J.first_tile[i] = (int)tiles;
+    tiles += (long long)jobs[i].batch * ceil_div(jobs[i].rows, 32) * ceil_div(jobs[i].cols, 32);
+    elems += (long long)jobs[i].batch * jobs[i].rows * jobs[i].cols;
+  }
+  for (int i = njobs; i <= kMaxTf32SplitJobs; ++i) J.first_tile[i] = (int)tiles;
+  if (tiles == 0) return RLX_OK;
+  RLX_LAUNCH_C(kclass, 0, 12.0 * elems, tf32_split_kernel, (unsigned)tiles, 256, 0, stream, J);
+  return RLX_OK;
 }
 
 }  // namespace rlx

@@ -99,8 +99,12 @@ static FwdPlan plan_forward(const rlx_ppo_dims& d, long long n) {
 
 constexpr int kHeadWgradRows = 64;
 
+// tf32 hi / lo copies of the weights the forward and dX GEMMs take as B, at the originals' pitches and per-net offsets
+enum { WS_W1_HI, WS_W1_LO, WS_W2_HI, WS_W2_LO, WS_W2T_HI, WS_W2T_LO, WS_COUNT };
+
 struct TrainPlan {
   size_t off_H1, off_H2, off_dZ2, off_dZ1, off_dhead, off_headpart, off_part1, off_rs1, off_part2, off_part3, off_norm, off_barrier, off_P, off_X, off_ratio, total;
+  size_t off_wsplit[WS_COUNT];
   int max_s1, max_s2, max_s3;
   int head_blocks, wgrad_chunks, norm_blocks, head_npart;
 };
@@ -140,6 +144,7 @@ static TrainPlan plan_train(const rlx_ppo_dims& d, long long m) {
   take(P.off_P, (size_t)make_layout(d).total());                          // bf16-autocast mode: rounded parameter copy
   take(P.off_X, (size_t)m * (size_t)(ceil_div(O + 1, 4) * 4));             // ... and rounded copy of the minibatch states (pitch <= obs + 4)
   take(P.off_ratio, (size_t)m);                                           // ESPO median: |ratio - 1| per row
+  for (int i = 0; i < WS_COUNT; ++i) take(P.off_wsplit[i], i < WS_W2_HI ? (size_t)(2 * H * O) : (size_t)(2 * H * H));
   P.total = o;
   return P;
 }
@@ -155,9 +160,24 @@ static size_t head_smem_bytes(const rlx_ppo_dims& d, bool train) {
   return s;
 }
 
-// hidden layers: H1 = tanh(X W1cat^T + b1cat), H2 = tanh(H1 (blockdiag W2)^T + b2cat).  ldx = row pitch of X.
+// The minibatch update's copies (pointers into the workspace); split_weights refreshes them from the parameters.
+struct SplitWeights {
+  const float* p[WS_COUNT];
+};
+static int split_weights(const PpoLayout& L, const float* params, void* ws, const TrainPlan& P, SplitWeights& sw, cudaStream_t st) {
+  const int H = L.H;
+  float* w[WS_COUNT];
+  for (int i = 0; i < WS_COUNT; ++i) sw.p[i] = w[i] = ws_ptr<float>(ws, P.off_wsplit[i]);
+  const Tf32SplitJob jobs[3] = {{params + L.off[W1P], w[WS_W1_HI], w[WS_W1_LO], 1, 2 * H, L.obs, 0},
+                                {params + L.off[W2P], w[WS_W2_HI], w[WS_W2_LO], 1, 2 * H, H, 0},
+                                {params + L.off[W2P], w[WS_W2T_HI], w[WS_W2T_LO], 2, H, H, 1}};
+  return tf32_split(jobs, 3, KC_GEMM_FWD, st);  // a few microseconds, charged to the forward GEMMs
+}
+
+// hidden layers: H1 = tanh(X W1cat^T + b1cat), H2 = tanh(H1 (blockdiag W2)^T + b2cat).  ldx = row pitch of X.  sw: tf32 hi / lo copies of
+// W1cat and W2 (wgmma engine, fp32 mode), or null.
 static int mlp_hidden_forward(const rlx_ppo_dims& d, const PpoLayout& L, const float* params, const float* X, long long ldx, long long rows,
-                              float* H1, float* H2, cudaStream_t stream, int bf16 = 0) {
+                              float* H1, float* H2, cudaStream_t stream, int bf16 = 0, const SplitWeights* sw = nullptr) {
   const int H = L.H;
   const bool tc = use_tc(d);
   GemmP g{};
@@ -166,10 +186,12 @@ static int mlp_hidden_forward(const rlx_ppo_dims& d, const PpoLayout& L, const f
   g.lda = (int)ldx; g.ldb = L.obs; g.ldc = 2 * H;
   g.splits = 1; g.kchunk = (int)(ceil_div(L.obs, 8) * 8);
   g.bf16 = bf16;
+  if (sw) { g.b_hi = sw->p[WS_W1_HI]; g.b_lo = sw->p[WS_W1_LO]; }
   int rc = run_gemm<true, true, EPI_BIAS_TANH>(tc, g, 1, stream, KC_GEMM_FWD, rows, 2 * H);
   if (rc) return rc;
   GemmP g2{};
   g2.A = H1; g2.B = params + L.off[W2P]; g2.C = H2; g2.bias = params + L.off[B2P];
+  if (sw) { g2.b_hi = sw->p[WS_W2_HI]; g2.b_lo = sw->p[WS_W2_LO]; }
   g2.M = (int)rows; g2.N = H; g2.K = H;
   g2.lda = 2 * H; g2.ldb = H; g2.ldc = 2 * H;
   g2.sA = H; g2.sB = (long long)H * H; g2.sC = H; g2.sBias = H;
@@ -501,9 +523,10 @@ static int launch_head_wgrad(const PpoLayout& L, const TrainPlan& P, long long m
   return RLX_OK;
 }
 
-// hidden layers backward: dW2, dZ1, dW1 | db1 (split over rows; s1 / s2 = split counts of the dW1 | db1 / dW2 partials)
+// hidden layers backward: dW2, dZ1, dW1 | db1 (split over rows; s1 / s2 = split counts of the dW1 | db1 / dW2 partials).  sw: as in
+// mlp_hidden_forward (dZ1 takes W2^T)
 static int launch_hidden_backward(const PpoLayout& L, const TrainPlan& P, const float* params, const float* states, long long ldx, bool ones_col,
-                                  long long m, bool tc, int bf16, void* ws, cudaStream_t st, int& s1, int& s2) {
+                                  long long m, bool tc, int bf16, const SplitWeights* sw, void* ws, cudaStream_t st, int& s1, int& s2) {
   const int H = L.H, O = L.obs;
   float* H1 = ws_ptr<float>(ws, P.off_H1);
   float* dZ2 = ws_ptr<float>(ws, P.off_dZ2);
@@ -531,6 +554,7 @@ static int launch_hidden_backward(const PpoLayout& L, const TrainPlan& P, const 
   gd.lda = 2 * H; gd.ldb = H; gd.ldc = 2 * H; gd.ldaux = 2 * H;
   gd.sA = H; gd.sB = (long long)H * H; gd.sC = H; gd.sAux = H;
   gd.splits = 1; gd.kchunk = (int)(ceil_div(H, 8) * 8);
+  if (sw) { gd.b_hi = sw->p[WS_W2T_HI]; gd.b_lo = sw->p[WS_W2T_LO]; }  // W2^T [i][o] is the K-major form of W2 here (square: same pitch)
   rc = run_gemm<true, false, EPI_DTANH>(tc, gd, 2, st, KC_GEMM_DX, m, H);
   if (rc) return rc;
   // ---- dW1cat | db1cat : part1[split][o][i] = sum_rows dZ1[r, o] * X[r, i];  db1[o] = sum_rows dZ1[r, o]
@@ -623,13 +647,22 @@ static int minibatch_fwdbwd(const rlx_ppo_minibatch_args* a, void* stream, bool 
       rc = round_inputs_bf16(L, params, states, m * ldx, ws_ptr<float>(ws, P.off_P), ws_ptr<float>(ws, P.off_X), st);
       if (rc) return rc;
     }
-    rc = mlp_hidden_forward(a->dims, L, params, states, ldx, m, ws_ptr<float>(ws, P.off_H1), ws_ptr<float>(ws, P.off_H2), st, bf16);
+    // wgmma engine, fp32: split the weights once here rather than in every tile of the forward and dX GEMMs.  Made from the current
+    // parameters on every call, so whatever wrote them last (Adam, init, a checkpoint load, a broadcast) is what the GEMMs see.
+    SplitWeights sw{};
+    const bool presplit = tc && !bf16;
+    if (presplit) {
+      rc = split_weights(L, params, ws, P, sw, st);
+      if (rc) return rc;
+    }
+    rc = mlp_hidden_forward(a->dims, L, params, states, ldx, m, ws_ptr<float>(ws, P.off_H1), ws_ptr<float>(ws, P.off_H2), st, bf16,
+                            presplit ? &sw : nullptr);
     if (rc) return rc;
     head_blocks = launch_train_head(a, L, P, params, bf16, st);
     if (head_blocks < 0) return head_blocks;
     rc = launch_head_wgrad(L, P, m, tc, bf16, ws, st, w3);
     if (rc) return rc;
-    rc = launch_hidden_backward(L, P, params, states, ldx, a->states_ones_col, m, tc, bf16, ws, st, s1, s2);
+    rc = launch_hidden_backward(L, P, params, states, ldx, a->states_ones_col, m, tc, bf16, presplit ? &sw : nullptr, ws, st, s1, s2);
     if (rc) return rc;
   }
   rc = launch_grad_reduce(make_grad_reduce(a, L, P, head_blocks, w3, s1, s2, fuse_norms), st);
@@ -767,15 +800,19 @@ extern "C" int rlx_ppo_update_epoch_sharded_f32(const rlx_ppo_minibatch_args* fi
 // Test hook: one plain GEMM through either engine (single batch, no split): layout 0 = A k-major, B k-major (C = A B^T);
 // 1 = A k-major, B n-major (C = A B); 2 = A m-major, B n-major (C = A^T B, A is [K, M]).  Epilogue 0 none, 1 bias+tanh, 3 bias+relu,
 // 5 bias (layout 0), 2 tanh', 4 relu' (layout 1, aux [M, ldaux]); 6 (layout 2, wgmma engine only) the transposed store with an extra row:
-// rows 0 .. M-2 of the product go transposed into C [N, ldc], row M-1 into row N of C.
+// rows 0 .. M-2 of the product go transposed into C [N, ldc], row M-1 into row N of C.  Pre-split B (wgmma engine only): layout 3 = layout 0
+// with epilogue 1, B [N, ldb] split by tf32_split into a scratch copy first; 4 = layout 1 with epilogue 2, B [K, ldb] split and transposed
+// into a [ldb, K] copy first (K a multiple of 4) - the forward and dX GEMMs of the PPO update.
 extern "C" int rlx_debug_gemm_f32(int engine, int layout, int epilogue, int64_t M, int64_t N, int64_t K, const float* A, int64_t lda,
                                   const float* B, int64_t ldb, float* C, int64_t ldc, const float* bias, const float* aux, int64_t ldaux,
                                   void* stream) {
   RLX_CHECK_ARG(A && B && C && M > 0 && N > 0 && K > 0, "bad arguments");
   RLX_CHECK_ARG(engine == 0 || engine == 1, "unknown engine (0 = SIMT, 1 = wgmma tensor cores)");
   const bool bias_epi = epilogue == 1 || epilogue == 3 || epilogue == 5, aux_epi = epilogue == 2 || epilogue == 4;
-  RLX_CHECK_ARG((epilogue == 0) || (bias_epi && layout == 0 && bias) || (aux_epi && layout == 1 && aux) ||
-                    (epilogue == 6 && layout == 2 && engine == 1 && M >= 2),
+  const bool presplit = layout == 3 || layout == 4;
+  RLX_CHECK_ARG((epilogue == 0 && !presplit) || (bias_epi && layout == 0 && bias) || (aux_epi && layout == 1 && aux) ||
+                    (epilogue == 6 && layout == 2 && engine == 1 && M >= 2) ||
+                    (engine == 1 && layout == 3 && epilogue == 1 && bias) || (engine == 1 && layout == 4 && epilogue == 2 && aux && K % 4 == 0),
                 "unsupported epilogue/layout");
   GemmP g{};
   g.A = A; g.B = B; g.C = C; g.bias = bias; g.aux = aux;
@@ -783,6 +820,20 @@ extern "C" int rlx_debug_gemm_f32(int engine, int layout, int epilogue, int64_t 
   g.lda = (int)lda; g.ldb = (int)ldb; g.ldc = (int)ldc; g.ldaux = (int)ldaux;
   g.splits = 1; g.kchunk = (int)(ceil_div(K, 8) * 8);
   cudaStream_t st = (cudaStream_t)stream;
+  if (presplit) {
+    const int rows = (int)(layout == 3 ? N : K);
+    float* hi = nullptr;
+    RLX_CHECK_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&hi), 2 * sizeof(float) * rows * ldb, st));
+    const Tf32SplitJob job{B, hi, hi + rows * ldb, 1, rows, (int)ldb, layout == 4};
+    int rc = tf32_split(&job, 1, KC_OTHER, st);
+    if (rc == RLX_OK) {
+      g.b_hi = job.hi; g.b_lo = job.lo;
+      if (layout == 4) g.ldb = (int)K;  // pitch of the transposed copy
+      rc = tc_gemm(g, true, layout == 3, epilogue, 1, KC_OTHER, M, layout == 3 ? N : K, st);
+    }
+    RLX_CHECK_CUDA(cudaFreeAsync(hi, st));
+    return rc;
+  }
   const bool a_k = layout != 2, b_k = layout == 0;
   const long long a_rows = a_k ? M : K, b_rows = b_k ? N : K;
   if (engine == 1) {
@@ -799,6 +850,13 @@ extern "C" int rlx_debug_gemm_f32(int engine, int layout, int epilogue, int64_t 
   if (layout == 1 && epilogue == 4) return launch_sgemm<true, false, EPI_DRELU>(g, 1, st);
   if (layout == 1) return launch_sgemm<true, false, EPI_NONE>(g, 1, st);
   return launch_sgemm<false, false, EPI_NONE>(g, 1, st);
+}
+
+// Test hook: the tf32 hi / lo split the minibatch update makes of its weights (tf32_split), of src [batch][rows][cols]
+extern "C" int rlx_debug_tf32_split_f32(const float* src, int64_t batch, int64_t rows, int64_t cols, int trans, float* hi, float* lo, void* stream) {
+  RLX_CHECK_ARG(src && hi && lo && batch > 0 && rows > 0 && cols > 0 && batch * rows * cols < (1LL << 31), "bad arguments");
+  const Tf32SplitJob job{src, hi, lo, (int)batch, (int)rows, (int)cols, trans ? 1 : 0};
+  return tf32_split(&job, 1, KC_OTHER, (cudaStream_t)stream);
 }
 
 extern "C" int rlx_set_head_engine(int engine) {
