@@ -48,7 +48,9 @@ int rlx_timing_begin(void);
 int rlx_timing_end(double* ms, uint64_t* launches, double* flops, double* bytes);
 const char* rlx_kernel_class_name(int cls);
 /* GEMM engine used by the MLP entry points: 0 = fp32 SIMT (FFMA), 1 = wgmma 3xTF32 (tensor cores, register accumulators).
- * Returns the engine actually in effect (a request for 1 falls back to 0 with an error string if the shape is unsupported). */
+ * Sets a process-wide preference and returns it; any other value is refused with an error string and the previous choice returned.
+ * Under 1 each call still decides on its own, without an error: a network whose shape the wgmma engine does not take (hidden not a
+ * multiple of 128 in 128..1024, or obs_dim below 32 or not a multiple of 4), and any single GEMM it does not cover, runs on the SIMT engine. */
 int rlx_set_gemm_engine(int engine);
 int rlx_get_gemm_engine(void);
 /* The same choice for the dense layers of the FastSAC and PPO+LSTM entry points (their own switch: these paths were validated on the SIMT
@@ -56,6 +58,14 @@ int rlx_get_gemm_engine(void);
  * engine (e.g. the 101-column logits of the C51 critics, whose row pitch is not a multiple of 16 bytes).  Default 0.  Returns the value in effect. */
 int rlx_set_aux_gemm_engine(int engine);
 uint64_t rlx_aux_tc_gemm_count(void);     /* GEMMs of those two paths that ran on the wgmma engine since load */
+/* Which GEMM kernels the library launched, counted on the host after each successful launch since load / the last reset (so a test can
+ * prove which engine served a call).  Slot s < 256: the wgmma engine's tc_gemm_kernel instance with template arguments
+ * s = A_KMAJ | B_KMAJ << 1 | EPI << 2 | BF16 << 5 | TRANS << 6 | SPLIT_B << 7 (EPI 0 none, 1 bias+tanh, 2 tanh', 3 bias+relu, 4 relu',
+ * 5 bias); 256 tf32_split_kernel; 257 the SIMT engine's sgemm_kernel; 258 the SIMT head weight-gradient kernels of the PPO update.
+ * Any other slot reads 0. */
+#define RLX_GEMM_PATH_SLOTS 259
+uint64_t rlx_gemm_path_count(int slot);
+void rlx_reset_gemm_path_counts(void);
 
 /* Test hook: one plain fp32 GEMM through either engine (0 = SIMT, 1 = wgmma; any other value is RLX_ERR_INVALID_ARG).  layout 0: C[M,N] = A[M,K] B[N,K]^T; 1: C = A[M,K] B[K,N];
  * 2: C = A[K,M]^T B[K,N].  epilogue 0 none, 1 tanh(x + bias[n]) (layout 0), 2 x * (1 - aux[m,n]^2) (layout 1).  Layouts 3 / 4 (wgmma engine,

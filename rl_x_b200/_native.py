@@ -174,6 +174,8 @@ _SIGNATURES = {
     "rlx_last_error_string": (C.c_char_p, []),
     "rlx_set_aux_gemm_engine": (C.c_int, [C.c_int]),
     "rlx_aux_tc_gemm_count": (C.c_uint64, []),
+    "rlx_gemm_path_count": (C.c_uint64, [C.c_int]),
+    "rlx_reset_gemm_path_counts": (None, []),
     "rlx_launch_count": (C.c_uint64, []),
     "rlx_reset_launch_count": (None, []),
     "rlx_add_launch_count": (None, [C.c_uint64]),

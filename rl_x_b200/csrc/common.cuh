@@ -24,6 +24,16 @@ extern int g_autocast_bf16;
 
 inline void count_launch(uint64_t n = 1) { g_launch_count.fetch_add(n, std::memory_order_relaxed); }
 
+// Launches of each GEMM path (rlx_gemm_path_count): slot tc_path_slot(...) per tc_gemm_kernel instance, then tf32_split, the SIMT GEMM and the
+// SIMT head weight-gradient kernels.  Counted on the host right after a successful launch.
+enum { GP_TF32_SPLIT = 256, GP_SGEMM, GP_HEAD_WGRAD_SIMT, GP_COUNT };
+static_assert(GP_COUNT == RLX_GEMM_PATH_SLOTS, "GEMM path slots out of sync with rlx_b200.h");
+extern std::atomic<uint64_t> g_gemm_path[GP_COUNT];
+inline void count_gemm_path(int slot) { g_gemm_path[slot].fetch_add(1, std::memory_order_relaxed); }
+constexpr int tc_path_slot(bool a_kmaj, bool b_kmaj, int epi, bool bf16, bool trans, bool split_b) {
+  return (a_kmaj ? 1 : 0) | (b_kmaj ? 2 : 0) | (epi << 2) | (bf16 ? 32 : 0) | (trans ? 64 : 0) | (split_b ? 128 : 0);
+}
+
 #define RLX_CHECK_ARG(cond, msg)                                  \
   do {                                                            \
     if (!(cond)) {                                                \

@@ -214,6 +214,7 @@ int launch_sgemm(const GemmP& p, int batch, cudaStream_t stream, int kclass = KC
   } else {
     RLX_LAUNCH_C(kclass, flops, bytes, (sgemm_kernel<A_KMAJ, B_KMAJ, EPI, false>), grid, 256, 0, stream, p);
   }
+  count_gemm_path(GP_SGEMM);
   return RLX_OK;
 }
 

@@ -462,6 +462,7 @@ static int launch_cfg(const TcOperand& A, const TcOperand& B, TcParams p, int kc
   const double flops = 2.0 * p.M * p.N * (double)p.K * p.batch;
   const double bytes = 4.0 * p.batch * ((double)p.M * p.K + (SPLIT_B ? 2.0 : 1.0) * p.N * p.K + (double)p.M * p.N * p.splits);
   RLX_LAUNCH_C(kclass, flops, bytes, kern, grid, NUM_THREADS, smem, stream, ta, tb, tb_lo, p);
+  count_gemm_path(tc_path_slot(A_KMAJ, B_KMAJ, EPI, BF16, TRANS, SPLIT_B));
   return RLX_OK;
 }
 
@@ -619,6 +620,7 @@ int tf32_split(const Tf32SplitJob* jobs, int njobs, int kclass, cudaStream_t str
   for (int i = njobs; i <= kMaxTf32SplitJobs; ++i) J.first_tile[i] = (int)tiles;
   if (tiles == 0) return RLX_OK;
   RLX_LAUNCH_C(kclass, 0, 12.0 * elems, tf32_split_kernel, (unsigned)tiles, 256, 0, stream, J);
+  count_gemm_path(GP_TF32_SPLIT);
   return RLX_OK;
 }
 

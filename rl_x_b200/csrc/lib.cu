@@ -9,6 +9,7 @@ std::atomic<uint64_t> g_launch_count{0};
 int g_gemm_engine = 0;
 int g_aux_gemm_engine = 0;  // FastSAC / PPO+LSTM dense layers (rlx_set_aux_gemm_engine)
 std::atomic<uint64_t> g_aux_tc_gemms{0};
+std::atomic<uint64_t> g_gemm_path[GP_COUNT];
 int g_autocast_bf16 = 0;
 
 void set_error(const char* fmt, ...) {
@@ -60,6 +61,10 @@ extern "C" void rlx_reset_launch_count(void) { rlx::g_launch_count.store(0); }
 extern "C" void rlx_add_launch_count(uint64_t n) { rlx::g_launch_count.fetch_add(n); }
 extern "C" int rlx_get_gemm_engine(void) { return rlx::g_gemm_engine; }
 extern "C" uint64_t rlx_aux_tc_gemm_count(void) { return rlx::g_aux_tc_gemms.load(); }
+extern "C" uint64_t rlx_gemm_path_count(int slot) { return (slot >= 0 && slot < rlx::GP_COUNT) ? rlx::g_gemm_path[slot].load() : 0; }
+extern "C" void rlx_reset_gemm_path_counts(void) {
+  for (auto& c : rlx::g_gemm_path) c.store(0);
+}
 extern "C" int rlx_set_aux_gemm_engine(int engine) {
   if (engine == 0 || engine == 1) rlx::g_aux_gemm_engine = engine;
   else rlx::set_error("rlx_set_aux_gemm_engine: unknown engine %d", engine);

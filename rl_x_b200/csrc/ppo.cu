@@ -486,6 +486,7 @@ static int launch_head_wgrad(const PpoLayout& L, const TrainPlan& P, long long m
       RLX_CHECK_CUDA(cudaFuncSetAttribute(ppo_head_wgrad_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem));
       RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad_kernel<64>, wg, 256, wsmem, st, w);
     }
+    count_gemm_path(GP_HEAD_WGRAD_SIMT);
     w3 = chunked_w3(L, part3, wgrad_chunks);
     return RLX_OK;
   }
@@ -519,6 +520,7 @@ static int launch_head_wgrad(const PpoLayout& L, const TrainPlan& P, long long m
   else if (A + 1 <= 20) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<20>, wgrad_chunks, wthreads, wsmem, st, w);
   else if (A + 1 <= 24) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<24>, wgrad_chunks, wthreads, wsmem, st, w);
   else RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<32>, wgrad_chunks, wthreads, wsmem, st, w);
+  count_gemm_path(GP_HEAD_WGRAD_SIMT);
   w3 = chunked_w3(L, part3, wgrad_chunks);
   return RLX_OK;
 }

@@ -60,7 +60,7 @@ def test_bf16_gae_bit_exact_vs_reference_golden():
         assert np.array_equal(adv.cpu().numpy(), g[f"iter{it}/advantages"]) and np.array_equal(ret.cpu().numpy(), g[f"iter{it}/returns"])
 
 
-@pytest.mark.parametrize("obs,act,hidden,n", [(11, 3, 64, 108), (376, 17, 256, 4096), (24, 5, 128, 300)])
+@pytest.mark.parametrize("obs,act,hidden,n", [(11, 3, 64, 108), (376, 17, 256, 4096), (24, 5, 128, 300), (32, 1, 128, 1000), (128, 4, 384, 2048)])
 def test_bf16_forward_vs_oracle(obs, act, hidden, n):
     k = _kern(obs, act, hidden)
     pol, cri = O.init_params(obs, act, hidden, std_dev=0.8, seed=obs + n)
@@ -123,7 +123,8 @@ def _grads_under_autocast(L, mb):
     return gp, gc, dict(pg_loss=pg.item(), critic_loss=closs.item(), approx_kl=kl.item(), clip_fraction=cf.item())
 
 
-@pytest.mark.parametrize("obs,act,hidden,m,ent", [(11, 3, 64, 40, 0.01), (376, 17, 256, 4096, 0.0), (376, 17, 256, 32768, 0.0), (24, 5, 128, 1000, 0.02)])
+@pytest.mark.parametrize("obs,act,hidden,m,ent", [(11, 3, 64, 40, 0.01), (376, 17, 256, 4096, 0.0), (376, 17, 256, 32768, 0.0), (24, 5, 128, 1000, 0.02),
+                                                 (32, 1, 128, 1000, 0.0), (128, 4, 384, 2048, 0.01)])  # the last two on the wgmma engine's BF16 instances
 def test_bf16_minibatch_gradients_vs_oracle_autograd(obs, act, hidden, m, ent):
     from rl_x_b200.algorithms.ppo.b200.kernels import make_hparams
     from test_gpu_parity import _random_minibatch, _run_fwdbwd
