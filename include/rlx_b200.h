@@ -53,9 +53,11 @@ const char* rlx_kernel_class_name(int cls);
  * multiple of 128 in 128..1024, or obs_dim below 32 or not a multiple of 4), and any single GEMM it does not cover, runs on the SIMT engine. */
 int rlx_set_gemm_engine(int engine);
 int rlx_get_gemm_engine(void);
-/* The same choice for the dense layers of the FastSAC and PPO+LSTM entry points (their own switch: these paths were validated on the SIMT
- * engine).  1 routes every GEMM whose layout / epilogue / alignment the wgmma engine covers to it and leaves the rest on the SIMT
- * engine (e.g. the 101-column logits of the C51 critics, whose row pitch is not a multiple of 16 bytes).  Default 0.  Returns the value in effect. */
+/* The same choice for the dense layers of the FastSAC, FastTD3 and PPO+LSTM entry points (their own switch: these paths were validated on the
+ * SIMT engine).  Like rlx_set_gemm_engine it is a preference: under 1 each GEMM still decides on its own, and one the wgmma engine does not
+ * cover - M or N below 64, K below 32, an operand base or row pitch that is not a multiple of 16 bytes (e.g. the 101-column logits of the
+ * C51 critics), a layout / epilogue pair without a kernel - runs on the SIMT engine without an error.  rlx_gemm_path_count tells which
+ * kernels a call launched.  Default 0.  Returns the value in effect. */
 int rlx_set_aux_gemm_engine(int engine);
 uint64_t rlx_aux_tc_gemm_count(void);     /* GEMMs of those two paths that ran on the wgmma engine since load */
 /* Which GEMM kernels the library launched, counted on the host after each successful launch since load / the last reset (so a test can

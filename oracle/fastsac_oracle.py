@@ -62,8 +62,8 @@ def _leaves(net):
     return out
 
 
-def _clone(net, grad):
-    f = (lambda t: t.clone().requires_grad_(True)) if grad else (lambda t: t.clone())
+def _clone(net, grad, dtype=torch.float32):
+    f = (lambda t: t.detach().to(dtype, copy=True).requires_grad_(True)) if grad else (lambda t: t.detach().to(dtype, copy=True))
     out = {"torso": [(f(w), f(b)) for w, b in net["torso"]]}
     for k in ("mean", "log_std", "head"):
         if k in net:
@@ -128,17 +128,20 @@ class Normalizer:
 
 class Learner:
     def __init__(self, pol, q1, q2, action_scale, lr, weight_decay, betas, gamma, tau, v_min, v_max, nr_atoms, target_entropy, alpha_init,
-                 log_std_min, log_std_max, clipped_double_q=False, max_grad_norm=-1.0):
+                 log_std_min, log_std_max, clipped_double_q=False, max_grad_norm=-1.0, dtype=torch.float32):
+        """dtype: the precision of every tensor of the learner (float32: the reference's; float64: the yardstick of the GPU tests, which pass
+        a float64 action_scale and float64 batches).  The tensors stay on the device of `pol`."""
         self.clipped, self.max_grad_norm = clipped_double_q, max_grad_norm
-        self.pol, self.q1, self.q2 = _clone(pol, True), _clone(q1, True), _clone(q2, True)
-        self.q1t, self.q2t = _clone(q1, False), _clone(q2, False)
-        self.log_alpha = torch.full((1,), math.log(alpha_init), requires_grad=True)
+        self.pol, self.q1, self.q2 = _clone(pol, True, dtype), _clone(q1, True, dtype), _clone(q2, True, dtype)
+        self.q1t, self.q2t = _clone(q1, False, dtype), _clone(q2, False, dtype)
+        dev = self.pol["mean"][0].device
+        self.log_alpha = torch.full((1,), math.log(alpha_init), dtype=dtype, device=dev, requires_grad=True)
         self.popt = torch.optim.AdamW(_leaves(self.pol), lr=lr, weight_decay=weight_decay, betas=betas)
         self.qopt = torch.optim.AdamW(_leaves(self.q1) + _leaves(self.q2), lr=lr, weight_decay=weight_decay, betas=betas)
         self.aopt = torch.optim.AdamW([self.log_alpha], lr=lr, weight_decay=weight_decay, betas=betas)
         self.action_scale, self.gamma, self.tau, self.v_min, self.v_max, self.nr_atoms = action_scale, gamma, tau, v_min, v_max, nr_atoms
         self.target_entropy, self.lsmin, self.lsmax = target_entropy, log_std_min, log_std_max
-        self.support = torch.linspace(v_min, v_max, nr_atoms)
+        self.support = torch.linspace(v_min, v_max, nr_atoms, dtype=dtype, device=dev)
 
     def critic_and_entropy_step(self, s, ns, a, r, dones, truncs, eff, eps_next):
         """fastsac.py:141-238, then the polyak update of :316-320."""
@@ -156,7 +159,7 @@ class Learner:
             up = torch.where(is_int & (lo0 == 0), up0 + 1, up0)
             d1 = F.softmax(q_forward(self.q1t, ns, na), dim=1)
             d2 = F.softmax(q_forward(self.q2t, ns, na), dim=1)
-            wl, wu = up.float() - b, b - lo.float()
+            wl, wu = up.to(b.dtype) - b, b - lo.to(b.dtype)
             proj1, proj2 = torch.zeros_like(d1), torch.zeros_like(d2)
             for proj, d in ((proj1, d1), (proj2, d2)):
                 proj.scatter_add_(1, lo, d * wl)

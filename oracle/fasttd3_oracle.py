@@ -49,8 +49,8 @@ def leaves(net):
     return [t for wb in net for t in wb]
 
 
-def _clone(net, grad):
-    f = (lambda t: t.clone().requires_grad_(True)) if grad else (lambda t: t.clone())
+def _clone(net, grad, dtype=torch.float32):
+    f = (lambda t: t.detach().to(dtype, copy=True).requires_grad_(True)) if grad else (lambda t: t.detach().to(dtype, copy=True))
     return [(f(w), f(b)) for w, b in net]
 
 
@@ -82,15 +82,17 @@ def act(pol, x, noise=None, noise_scales=None, low=None, high=None, clip_rescale
 
 class Learner:
     def __init__(self, pol, q1, q2, lr, weight_decay, gamma, tau, v_min, v_max, nr_atoms, smoothing_epsilon, smoothing_clip_value,
-                 clipped_double_q=True, max_grad_norm=-1.0):
+                 clipped_double_q=True, max_grad_norm=-1.0, dtype=torch.float32):
+        """dtype: the precision of every tensor of the learner (float32: the reference's; float64: the yardstick of the GPU tests, which pass
+        float64 batches).  The tensors stay on the device of `pol`."""
         self.clipped, self.max_grad_norm = clipped_double_q, max_grad_norm
-        self.pol, self.q1, self.q2 = _clone(pol, True), _clone(q1, True), _clone(q2, True)
-        self.q1t, self.q2t = _clone(q1, False), _clone(q2, False)
+        self.pol, self.q1, self.q2 = _clone(pol, True, dtype), _clone(q1, True, dtype), _clone(q2, True, dtype)
+        self.q1t, self.q2t = _clone(q1, False, dtype), _clone(q2, False, dtype)
         self.popt = torch.optim.AdamW(leaves(self.pol), lr=lr, weight_decay=weight_decay)
         self.qopt = torch.optim.AdamW(leaves(self.q1) + leaves(self.q2), lr=lr, weight_decay=weight_decay)
         self.gamma, self.tau, self.v_min, self.v_max, self.nr_atoms = gamma, tau, v_min, v_max, nr_atoms
         self.se, self.sclip = smoothing_epsilon, smoothing_clip_value
-        self.support = torch.linspace(v_min, v_max, nr_atoms)
+        self.support = torch.linspace(v_min, v_max, nr_atoms, dtype=dtype, device=self.pol[0][0].device)
 
     def set_lr(self, lr):
         for opt in (self.popt, self.qopt):
@@ -113,14 +115,15 @@ class Learner:
             up = torch.where(is_int & (lo0 == 0), up0 + 1, up0)
             d1 = F.softmax(q_forward(self.q1t, ns, na), dim=1)
             d2 = F.softmax(q_forward(self.q2t, ns, na), dim=1)
-            wl, wu = up.float() - b, b - lo.float()
+            wl, wu = up.to(b.dtype) - b, b - lo.to(b.dtype)
             proj1, proj2 = torch.zeros_like(d1), torch.zeros_like(d2)
             for proj, d in ((proj1, d1), (proj2, d2)):
                 proj.scatter_add_(1, lo, d * wl)
                 proj.scatter_add_(1, up, d * wu)
             q1_next_value = (proj1 * self.support).sum(1)
+            q2_next_value = (proj2 * self.support).sum(1)
+            self.next_values = (q1_next_value, q2_next_value)   # the two sides of the clipped double-Q selection, for the tests
             if self.clipped:
-                q2_next_value = (proj2 * self.support).sum(1)
                 proj1 = proj2 = torch.where(q1_next_value.unsqueeze(1) < q2_next_value.unsqueeze(1), proj1, proj2)
         l1 = -(proj1 * F.log_softmax(q_forward(self.q1, s, a), dim=1)).sum(1).mean()
         l2 = -(proj2 * F.log_softmax(q_forward(self.q2, s, a), dim=1)).sum(1).mean()

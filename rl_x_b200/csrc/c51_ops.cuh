@@ -178,6 +178,21 @@ static int adamw_step(float* p, const float* g, float* m, float* v, long long n,
 }
 
 // ------------------------------------------------------------------------------------------------------- GEMM helpers
+static __global__ void copy_kernel(const float* __restrict__ src, long long n, float* __restrict__ dst) {
+  const long long i = gtid();
+  if (i < n) dst[i] = src[i];
+}
+// *out = a network's parameter block as the GEMMs read it: P itself when its base is 16-byte aligned, else a copy of its n floats in `slot`
+// (16-byte aligned workspace).  The critics sit back to back in q_params, critic 2 at q_params + nq, and every segment is a multiple of 4
+// floats except the last bias (nr_atoms): with 101 atoms nq % 4 == 1, no weight of critic 2 can be a TMA operand in place, and aux_gemm would
+// run every GEMM that reads one on the SIMT engine.  The copy holds the same values, so the results do not depend on which one is read.
+static int aligned_params(const float* P, long long n, float* slot, const float** out, cudaStream_t st) {
+  *out = P;
+  if (((uintptr_t)P & 15) == 0) return RLX_OK;
+  RLX_FLAT_LAUNCH(copy_kernel, n, st, P, n, slot);
+  *out = slot;
+  return RLX_OK;
+}
 // torch Linear: Y[r, o] = epi(sum_i X[r, i] W[o, i] + b[o]), W row pitch ldw (= in unless a padded copy)
 template <int EPI = EPI_BIAS>
 static int lin_fwd(const float* X, int ldx, const float* W, int in, int out, const float* b, float* Y, int ldy, long long n, cudaStream_t st,

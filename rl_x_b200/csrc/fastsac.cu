@@ -46,7 +46,7 @@ static bool dims_ok(const rlx_fastsac_dims& d) { return d.obs_dim > 0 && d.act_d
 struct Acts { float *Z[3], *Y[3], *S[3]; };
 struct Ws {
   size_t pZ[3], pY[3], pS[3], qZ[2][3], qY[2][3], qS[2][3], XA, Mean, LsRaw, Act, Logp, Logits[2], Proj[2], dLogits, dZ, dY, dXA, dXA2, dAct, dMean, dLs,
-      RowA, RowB, Small, Part, Col, total;
+      RowA, RowB, Small, QP[2], Part, Col, total;
 };
 static Ws plan(const rlx_fastsac_dims& d, long long n_) {
   const size_t n = (size_t)n_, O = d.obs_dim, A = d.act_dim, K = d.nr_atoms;
@@ -60,6 +60,8 @@ static Ws plan(const rlx_fastsac_dims& d, long long n_) {
   for (int q = 0; q < 2; ++q) { take(w.Logits[q], n * K); take(w.Proj[q], n * K); }
   take(w.dLogits, n * K); take(w.dZ, n * 768); take(w.dY, n * 768); take(w.dXA, n * (O + A)); take(w.dXA2, n * (O + A)); take(w.dAct, n * A); take(w.dMean, n * A);
   take(w.dLs, n * A); take(w.RowA, n * 4); take(w.RowB, n * 4); take(w.Small, 64);
+  const size_t nq = (size_t)make_layout(d).q[RLX_FASTSAC_Q_NSEG];
+  take(w.QP[0], nq); take(w.QP[1], nq);   // aligned_params: a critic's parameter block when its base is not 16-byte aligned
   const size_t splits = (size_t)ceil_div((long long)n, kWgradRows);
   size_t biggest = std::max<size_t>((size_t)768 * (O + A), (size_t)768 * 384);
   biggest = std::max<size_t>(biggest, std::max<size_t>((size_t)512 * O, (size_t)K * 192));
@@ -356,8 +358,11 @@ extern "C" int rlx_fastsac_critic_update_f32(const rlx_fastsac_update_args* a, v
   // ---- target (no gradients): a' ~ pi(s'), both target networks on (s', a'), projection (fastsac.py:143-186)
   FS_TRY(policy_fwd(d, l, w, ws, a->policy_params, a->next_states, a->noise, a->action_scale, hp.log_std_min, hp.log_std_max, n, Act, Logp, st));
   RLX_FLAT_LAUNCH(concat_kernel, n * (O + A), st, a->next_states, Act, n, O, A, O + A, XA);
-  FS_TRY(q_fwd(d, l, a->q_target_params, XA, n, q0, ws + w.Logits[0], st));
-  FS_TRY(q_fwd(d, l, a->q_target_params + nq, XA, n, q1, ws + w.Logits[1], st));
+  for (int q = 0; q < 2; ++q) {
+    const float* QT;
+    FS_TRY(aligned_params(a->q_target_params + q * nq, nq, ws + w.QP[q], &QT, st));
+    FS_TRY(q_fwd(d, l, QT, XA, n, q == 0 ? q0 : q1, ws + w.Logits[q], st));
+  }
   RLX_FLAT_LAUNCH(c51_project_kernel, n, st, ws + w.Logits[0], ws + w.Logits[1], a->rewards, a->dones, a->truncations, a->effective_n_steps, Logp,
                   a->log_alpha, n, K, hp.gamma, hp.v_min, hp.v_max, hp.clipped_double_q != 0.f ? 1 : 0, ws + w.Proj[0], ws + w.Proj[1],
                   RowA /*q1_next_value*/);
@@ -368,9 +373,11 @@ extern "C" int rlx_fastsac_critic_update_f32(const rlx_fastsac_update_args* a, v
   const float inv_n = 1.f / (float)n;
   for (int q = 0; q < 2; ++q) {
     const Acts& aq = q == 0 ? q0 : q1;
-    FS_TRY(q_fwd(d, l, a->q_params + q * nq, XA, n, aq, ws + w.Logits[q], st));
+    const float* Q;
+    FS_TRY(aligned_params(a->q_params + q * nq, nq, ws + w.QP[q], &Q, st));
+    FS_TRY(q_fwd(d, l, Q, XA, n, aq, ws + w.Logits[q], st));
     RLX_FLAT_LAUNCH(ce_rows_kernel, n, st, ws + w.Logits[q], ws + w.Proj[q], n, K, inv_n, RowA + (1 + q) * n, ws + w.dLogits);
-    FS_TRY(q_bwd(d, l, w, ws, a->q_params + q * nq, a->q_grads + q * nq, XA, n, aq, ws + w.dLogits, nullptr, st));
+    FS_TRY(q_bwd(d, l, w, ws, Q, a->q_grads + q * nq, XA, n, aq, ws + w.dLogits, nullptr, st));
   }
   // sums: loss rows of both critics and the next log-probs (entropy = -next_log_probs)
   FS_TRY(colsum(RowA + n, 1, n, 1, Col, 1.f, 0.f, Small + 0, st));
@@ -406,22 +413,25 @@ extern "C" int rlx_fastsac_policy_update_f32(const rlx_fastsac_update_args* a, v
   FS_TRY(policy_fwd(d, l, w, ws, a->policy_params, a->states, a->noise, a->action_scale, hp.log_std_min, hp.log_std_max, n, Act, Logp, st));
   RLX_FLAT_LAUNCH(concat_kernel, n * (O + A), st, a->states, Act, n, O, A, O + A, XA);
   const int clipped = hp.clipped_double_q != 0.f ? 1 : 0;
+  const float* Qp[2];
   for (int q = 0; q < 2; ++q) {
-    FS_TRY(q_fwd(d, l, a->q_params + q * nq, XA, n, acts_q(ws, w, q), ws + w.Logits[q], st));
+    FS_TRY(aligned_params(a->q_params + q * nq, nq, ws + w.QP[q], &Qp[q], st));
+    FS_TRY(q_fwd(d, l, Qp[q], XA, n, acts_q(ws, w, q), ws + w.Logits[q], st));
     RLX_FLAT_LAUNCH(expect_rows_kernel, n, st, ws + w.Logits[q], n, K, hp.v_min, hp.v_max, RowA + (1 + q) * n, 0.f, (float*)nullptr);
   }
   for (int q = 0; q < 2; ++q) {
     const Acts aq = acts_q(ws, w, q);
+    const float* Q = Qp[q];
     // back through the critic to its input only (its own parameter gradients are not needed: the next critic update zeroes them)
     RLX_FLAT_LAUNCH(value_grad_rows_kernel, n, st, ws + w.Logits[q], RowA + (1 + q) * n, RowA + (2 - q) * n, n, K, hp.v_min, hp.v_max, clipped, inv_n,
                     ws + w.dLogits);
-    FS_TRY(lin_bwd_input(ws + w.dLogits, K, a->q_params + q * nq + l.q[12], 192, K, ws + w.dY, 192, n, st));
+    FS_TRY(lin_bwd_input(ws + w.dLogits, K, Q + l.q[12], 192, K, ws + w.dY, 192, n, st));
     for (int k = 2; k >= 0; --k) {
       const int W = kQW[k], in = k == 0 ? O + A : kQW[k - 1];
-      RLX_FLAT_LAUNCH(ln_silu_bwd_kernel, n, st, ws + w.dY, aq.Z[k], n, W, a->q_params + q * nq + l.q[4 * k + 2], a->q_params + q * nq + l.q[4 * k + 3],
+      RLX_FLAT_LAUNCH(ln_silu_bwd_kernel, n, st, ws + w.dY, aq.Z[k], n, W, Q + l.q[4 * k + 2], Q + l.q[4 * k + 3],
                       aq.S[k], ws + w.dZ);
       float* dst = k == 0 ? (q == 0 ? dXA : ws + w.dXA2) : ws + w.dY;
-      FS_TRY(lin_bwd_input(ws + w.dZ, W, a->q_params + q * nq + l.q[4 * k], in, W, dst, in, n, st));
+      FS_TRY(lin_bwd_input(ws + w.dZ, W, Q + l.q[4 * k], in, W, dst, in, n, st));
     }
   }
   // dAct = action columns of both critics' input gradients; back through the squashed-Gaussian head and the policy torso

@@ -39,7 +39,7 @@ static bool dims_ok(const rlx_fasttd3_dims& d) { return d.obs_dim > 0 && d.act_d
 static int xa_pitch(const rlx_fasttd3_dims& d) { return (int)align_up((size_t)(d.obs_dim + d.act_dim), 4); }
 
 struct Ws {
-  size_t pH[3], qH[2][3], XA, Act, Logits[2], Proj[2], dLogits, dA, dB, dXa[2], dAct, RowA, RowB, Zero, Small, W1[2], Part, Col, total;
+  size_t pH[3], qH[2][3], XA, Act, Logits[2], Proj[2], dLogits, dA, dB, dXa[2], dAct, RowA, RowB, Zero, Small, W1[2], QP[2], Part, Col, total;
 };
 static Ws plan(const rlx_fasttd3_dims& d, long long n_) {
   const size_t n = (size_t)n_, O = d.obs_dim, A = d.act_dim, K = d.nr_atoms, P = (size_t)xa_pitch(d);
@@ -54,6 +54,8 @@ static Ws plan(const rlx_fasttd3_dims& d, long long n_) {
   take(w.dLogits, n * K); take(w.dA, n * 1024); take(w.dB, n * 1024); take(w.dXa[0], n * A); take(w.dXa[1], n * A); take(w.dAct, n * A);
   take(w.RowA, n * 4); take(w.RowB, n * 4); take(w.Zero, n); take(w.Small, 64);
   take(w.W1[0], (size_t)kQW[0] * P); take(w.W1[1], (size_t)kQW[0] * P);
+  const size_t nq = (size_t)make_layout(d).q[RLX_FASTTD3_Q_NSEG];
+  take(w.QP[0], nq); take(w.QP[1], nq);   // aligned_params: a critic's parameter block when its base is not 16-byte aligned
   const size_t splits = (size_t)ceil_div((long long)n, kWgradRows);
   size_t biggest = std::max<size_t>((size_t)kQW[0] * P, (size_t)kQW[1] * kQW[0]);
   biggest = std::max<size_t>(biggest, std::max<size_t>((size_t)kPW[0] * O, (size_t)K * kQW[2]));
@@ -233,8 +235,11 @@ extern "C" int rlx_fasttd3_critic_update_f32(const rlx_fasttd3_update_args* a, v
   TD_TRY(policy_fwd(d, l, w, ws, a->policy_params, a->next_states, n, Act, st));
   RLX_FLAT_LAUNCH(smooth_target_action_kernel, n * A, st, Act, a->smoothing_noise, n * A, hp.smoothing_epsilon, hp.smoothing_clip_value);
   RLX_FLAT_LAUNCH(concat_kernel, n * (O + A), st, a->next_states, Act, n, O, A, ldx, XA);
-  TD_TRY(q_fwd(d, l, w, ws, a->q_target_params, 0, XA, n, q0, ws + w.Logits[0], st));
-  TD_TRY(q_fwd(d, l, w, ws, a->q_target_params + nq, 1, XA, n, q1, ws + w.Logits[1], st));
+  for (int q = 0; q < 2; ++q) {
+    const float* QT;
+    TD_TRY(aligned_params(a->q_target_params + q * nq, nq, ws + w.QP[q], &QT, st));
+    TD_TRY(q_fwd(d, l, w, ws, QT, q, XA, n, q == 0 ? q0 : q1, ws + w.Logits[q], st));
+  }
   // FastSAC's projection with a zero entropy term: r - discount * exp(0) * 0 == r
   RLX_FLAT_LAUNCH(fill_kernel, n, st, Zero, n, 0.f);
   RLX_FLAT_LAUNCH(fill_kernel, 1, st, Small + 8, 1LL, 0.f);
@@ -247,7 +252,8 @@ extern "C" int rlx_fasttd3_critic_update_f32(const rlx_fasttd3_update_args* a, v
   const float inv_n = 1.f / (float)n;
   for (int q = 0; q < 2; ++q) {
     const Hs& h = q == 0 ? q0 : q1;
-    const float* Q = a->q_params + q * nq;
+    const float* Q;
+    TD_TRY(aligned_params(a->q_params + q * nq, nq, ws + w.QP[q], &Q, st));
     TD_TRY(q_fwd(d, l, w, ws, Q, q, XA, n, h, ws + w.Logits[q], st));
     RLX_FLAT_LAUNCH(ce_rows_kernel, n, st, ws + w.Logits[q], ws + w.Proj[q], n, K, inv_n, RowA + (1 + q) * n, ws + w.dLogits);
     TD_TRY(mlp_bwd(Q, a->q_grads + q * nq, l.q, kQW, XA, ldx, O + A, h.h, K, ws + w.dLogits, n, ws + w.dA, ws + w.dB, ws + w.Part, ws + w.Col, st));
@@ -280,14 +286,16 @@ extern "C" int rlx_fasttd3_policy_update_f32(const rlx_fasttd3_update_args* a, v
   // a = pi(s); q = min / mean of E[q1], E[q2] on (s, a); L = -mean(q)   (fasttd3.py:106-120)
   TD_TRY(policy_fwd(d, l, w, ws, a->policy_params, a->states, n, Act, st));
   RLX_FLAT_LAUNCH(concat_kernel, n * (O + A), st, a->states, Act, n, O, A, ldx, XA);
+  const float* Qp[2];
   for (int q = 0; q < 2; ++q) {
-    TD_TRY(q_fwd(d, l, w, ws, a->q_params + q * nq, q, XA, n, hs_q(ws, w, q), ws + w.Logits[q], st));
+    TD_TRY(aligned_params(a->q_params + q * nq, nq, ws + w.QP[q], &Qp[q], st));
+    TD_TRY(q_fwd(d, l, w, ws, Qp[q], q, XA, n, hs_q(ws, w, q), ws + w.Logits[q], st));
     RLX_FLAT_LAUNCH(expect_rows_kernel, n, st, ws + w.Logits[q], n, K, hp.v_min, hp.v_max, RowA + (1 + q) * n, 0.f, (float*)nullptr);
   }
   // back through each critic to its action columns only (its parameter gradients are not needed: the next critic update zeroes them)
   for (int q = 0; q < 2; ++q) {
     const Hs h = hs_q(ws, w, q);
-    const float* Q = a->q_params + q * nq;
+    const float* Q = Qp[q];
     RLX_FLAT_LAUNCH(value_grad_rows_kernel, n, st, ws + w.Logits[q], RowA + (1 + q) * n, RowA + (2 - q) * n, n, K, hp.v_min, hp.v_max, clipped, inv_n,
                     ws + w.dLogits);
     float *dA = ws + w.dA, *dB = ws + w.dB;
