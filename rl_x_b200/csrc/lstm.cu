@@ -44,6 +44,18 @@ static Layout make_layout(const rlx_lstm_dims& d) {
   l.c[RLX_LSTM_CRITIC_NSEG] = o;
   return l;
 }
+// Offsets of the K-major copies PT / TC (rlx_lstm_ppo_minibatch_fwdbwd_f32): the segments of `l` in the same order, each starting on a
+// 16-byte boundary, so that a copy is a tensor-engine operand whatever the widths before it (with FiLM and an odd act, Wf itself is not).
+static Layout kmajor_layout(const Layout& l) {
+  Layout k;
+  long long o = 0;
+  for (int i = 0; i < RLX_LSTM_POLICY_NSEG; ++i) { o = (o + 3) / 4 * 4; k.p[i] = o; o += l.p[i + 1] - l.p[i]; }
+  k.p[RLX_LSTM_POLICY_NSEG] = o;
+  o = 0;
+  for (int i = 0; i < RLX_LSTM_CRITIC_NSEG; ++i) { o = (o + 3) / 4 * 4; k.c[i] = o; o += l.c[i + 1] - l.c[i]; }
+  k.c[RLX_LSTM_CRITIC_NSEG] = o;
+  return k;
+}
 static bool dims_ok(const rlx_lstm_dims& d) {
   return d.obs_dim > 0 && d.act_dim > 0 && d.act_dim <= 64 && d.hidden > 0 && d.enc_dim > 0 && d.enc_dim <= 1024 && d.lstm_dim > 0 && d.lstm_dim <= 1024 &&
          (d.options & ~(RLX_LSTM_OPT_FILM | RLX_LSTM_OPT_SHARED_ENCODER)) == 0;
@@ -79,8 +91,8 @@ static Ws plan(const rlx_lstm_dims& d, long long T, long long n) {
   const size_t film = is_film(d) ? 1 : 0;  // FiLM buffers (policy.py:102-105); zero-sized otherwise
   take(w.E2, film * R * E); take(w.LL, film * R * L); take(w.GB, film * R * 2 * E); take(w.dGB, film * R * 2 * E); take(w.dOL, film * R * E);
   take(w.dLL, film * R * L);
-  // K-major ([out, in]) copies of the dense kernels, at the offsets of the originals (rlx_lstm_ppo_minibatch_fwdbwd_f32 only)
-  const Layout lay = make_layout(d);
+  // K-major ([out, in]) copies of the dense kernels, at the offsets of kmajor_layout (rlx_lstm_ppo_minibatch_fwdbwd_f32 only)
+  const Layout lay = kmajor_layout(make_layout(d));
   take(w.TP, (size_t)lay.p[RLX_LSTM_POLICY_NSEG]); take(w.TC, (size_t)lay.c[RLX_LSTM_CRITIC_NSEG]);
   w.total = o * sizeof(float);
   return w;
@@ -624,15 +636,16 @@ extern "C" int rlx_lstm_ppo_minibatch_fwdbwd_f32(const rlx_lstm_minibatch_args* 
   //   torso input TI: [OL | LLp] (concat, width E + L) or OL * gamma + beta (FiLM, width E)
   const bool film = is_film(d), shared = is_shared(d);
   const int TIW = film ? E : EL;
-  // K-major copies of the dense kernels (see dense_fwd_t): PT / CT mirror P / Cp segment by segment
+  // K-major copies of the dense kernels (see dense_fwd_t): PT / CT hold P / Cp segment by segment, at the aligned offsets of kmajor_layout
+  const Layout kl = kmajor_layout(l);
   float *PT = ws + w.TP, *CT = ws + w.TC;
   {
     const struct { int seg, in, out; bool on; } pk[] = {{WE1, O, E, true}, {WE2, O, E, !shared}, {WI, E, 4 * L, true}, {WT1, TIW, H, true}, {WT2, H, H, true},
                                                         {WM, H, A, true}, {WF, L, 2 * E, film}};
     for (const auto& k : pk)
-      if (k.on) LSTM_LAUNCH(transpose_kernel, (long long)k.in * k.out, st, P + l.p[k.seg], k.in, k.out, PT + l.p[k.seg]);
+      if (k.on) LSTM_LAUNCH(transpose_kernel, (long long)k.in * k.out, st, P + l.p[k.seg], k.in, k.out, PT + kl.p[k.seg]);
     const struct { int seg, in, out; } ck[] = {{WC1, O, H}, {WC2, H, H}, {WC3, H, 1}};
-    for (const auto& k : ck) LSTM_LAUNCH(transpose_kernel, (long long)k.in * k.out, st, Cp + l.c[k.seg], k.in, k.out, CT + l.c[k.seg]);
+    for (const auto& k : ck) LSTM_LAUNCH(transpose_kernel, (long long)k.in * k.out, st, Cp + l.c[k.seg], k.in, k.out, CT + kl.c[k.seg]);
   }
   float* OL = shared ? E1 : (film ? ws + w.E2 : TI);
   const int ldOL = (shared || film) ? E : EL;
@@ -641,16 +654,16 @@ extern "C" int rlx_lstm_ppo_minibatch_fwdbwd_f32(const rlx_lstm_minibatch_args* 
 
   // ================================================================ forward
   // encoders (policy.py:79-92): Z = X We + be; E = tanh(LN(Z))
-  LSTM_TRY(dense_fwd_t<EPI_BIAS>(X, O, PT + l.p[WE1], O, E, P + l.p[BE1], Z1, E, R, st));
+  LSTM_TRY(dense_fwd_t<EPI_BIAS>(X, O, PT + kl.p[WE1], O, E, P + l.p[BE1], Z1, E, R, st));
   LSTM_LAUNCH(ln_tanh_fwd_kernel, R, st, Z1, E, R, E, P + l.p[G1], P + l.p[N1], E1, E, S1);
   if (!shared) {
-    LSTM_TRY(dense_fwd_t<EPI_BIAS>(X, O, PT + l.p[WE2], O, E, P + l.p[BE2], Z2, E, R, st));
+    LSTM_TRY(dense_fwd_t<EPI_BIAS>(X, O, PT + kl.p[WE2], O, E, P + l.p[BE2], Z2, E, R, st));
     LSTM_LAUNCH(ln_tanh_fwd_kernel, R, st, Z2, E, R, E, P + l.p[G2], P + l.p[N2], OL, ldOL, S2);
   } else if (!film) {
     LSTM_LAUNCH(cols_kernel<false>, R * E, st, E1, E, R, E, TI, EL);
   }
   // input-side gate pre-activations of all steps at once, then the recurrence, one launch per step (policy.py:115-146)
-  LSTM_TRY(dense_fwd_t<EPI_NONE>(E1, E, PT + l.p[WI], E, 4 * L, nullptr, Gi, 4 * L, R, st));
+  LSTM_TRY(dense_fwd_t<EPI_NONE>(E1, E, PT + kl.p[WI], E, 4 * L, nullptr, Gi, 4 * L, R, st));
   const SeqCfg seq = seq_cfg(L);
   if (seq.ok) {
     RLX_BLOCK_LAUNCH(lstm_seq_fwd_kernel, ceil_div(n, seq.epb), seq.threads, seq.smem_fwd, st, Gi, P + l.p[WH], P + l.p[BH], a->init_h, a->init_c, a->dones,
@@ -668,16 +681,16 @@ extern "C" int rlx_lstm_ppo_minibatch_fwdbwd_f32(const rlx_lstm_minibatch_args* 
   // decode (policy.py:95-112): lstm latent = tanh(LN(h)); combination; torso; mean head
   LSTM_LAUNCH(ln_tanh_fwd_kernel, R, st, Hall, L, R, L, P + l.p[GL], P + l.p[NL], LLp, ldLL, SL);
   if (film) {
-    LSTM_TRY(dense_fwd_t<EPI_BIAS>(LLp, L, PT + l.p[WF], L, 2 * E, P + l.p[BF], ws + w.GB, 2 * E, R, st));
+    LSTM_TRY(dense_fwd_t<EPI_BIAS>(LLp, L, PT + kl.p[WF], L, 2 * E, P + l.p[BF], ws + w.GB, 2 * E, R, st));
     LSTM_LAUNCH(film_fwd_kernel, R * E, st, OL, ldOL, ws + w.GB, R, E, TI);
   }
-  LSTM_TRY(dense_fwd_t<EPI_BIAS_TANH>(TI, TIW, PT + l.p[WT1], TIW, H, P + l.p[BT1], T1, H, R, st));
-  LSTM_TRY(dense_fwd_t<EPI_BIAS_TANH>(T1, H, PT + l.p[WT2], H, H, P + l.p[BT2], T2, H, R, st));
-  LSTM_TRY(dense_fwd_t<EPI_BIAS>(T2, H, PT + l.p[WM], H, A, P + l.p[BM], Mean, A, R, st));
+  LSTM_TRY(dense_fwd_t<EPI_BIAS_TANH>(TI, TIW, PT + kl.p[WT1], TIW, H, P + l.p[BT1], T1, H, R, st));
+  LSTM_TRY(dense_fwd_t<EPI_BIAS_TANH>(T1, H, PT + kl.p[WT2], H, H, P + l.p[BT2], T2, H, R, st));
+  LSTM_TRY(dense_fwd_t<EPI_BIAS>(T2, H, PT + kl.p[WM], H, A, P + l.p[BM], Mean, A, R, st));
   // critic (critic.py:22-30)
-  LSTM_TRY(dense_fwd_t<EPI_BIAS_TANH>(X, O, CT + l.c[WC1], O, H, Cp + l.c[BC1], C1, H, R, st));
-  LSTM_TRY(dense_fwd_t<EPI_BIAS_TANH>(C1, H, CT + l.c[WC2], H, H, Cp + l.c[BC2], C2, H, R, st));
-  LSTM_TRY(dense_fwd_t<EPI_BIAS>(C2, H, CT + l.c[WC3], H, 1, Cp + l.c[BC3], V, 1, R, st));
+  LSTM_TRY(dense_fwd_t<EPI_BIAS_TANH>(X, O, CT + kl.c[WC1], O, H, Cp + l.c[BC1], C1, H, R, st));
+  LSTM_TRY(dense_fwd_t<EPI_BIAS_TANH>(C1, H, CT + kl.c[WC2], H, H, Cp + l.c[BC2], C2, H, R, st));
+  LSTM_TRY(dense_fwd_t<EPI_BIAS>(C2, H, CT + kl.c[WC3], H, 1, Cp + l.c[BC3], V, 1, R, st));
 
   // ================================================================ loss (ppo_lstm.py:146-172) and head gradients
   const float inv_R = 1.f / (float)R;
@@ -691,13 +704,13 @@ extern "C" int rlx_lstm_ppo_minibatch_fwdbwd_f32(const rlx_lstm_minibatch_args* 
   // ================================================================ backward: policy head and torso
   LSTM_TRY(dense_bwd_weight(T2, H, dMean, A, H, A, R, Part, gP + l.p[WM], st));
   LSTM_TRY(colsum(dMean, A, R, A, Col, 1.f, 0.f, gP + l.p[BM], st));
-  LSTM_TRY(dense_bwd_input_t<EPI_DTANH>(dMean, A, PT + l.p[WM], H, A, T2, H, dT2, H, R, st));          // dL/d(pre-tanh of torso 2)
+  LSTM_TRY(dense_bwd_input_t<EPI_DTANH>(dMean, A, PT + kl.p[WM], H, A, T2, H, dT2, H, R, st));          // dL/d(pre-tanh of torso 2)
   LSTM_TRY(dense_bwd_weight(T1, H, dT2, H, H, H, R, Part, gP + l.p[WT2], st));
   LSTM_TRY(colsum(dT2, H, R, H, Col, 1.f, 0.f, gP + l.p[BT2], st));
-  LSTM_TRY(dense_bwd_input_t<EPI_DTANH>(dT2, H, PT + l.p[WT2], H, H, T1, H, dT1, H, R, st));
+  LSTM_TRY(dense_bwd_input_t<EPI_DTANH>(dT2, H, PT + kl.p[WT2], H, H, T1, H, dT1, H, R, st));
   LSTM_TRY(dense_bwd_weight(TI, TIW, dT1, H, TIW, H, R, Part, gP + l.p[WT1], st));
   LSTM_TRY(colsum(dT1, H, R, H, Col, 1.f, 0.f, gP + l.p[BT1], st));
-  LSTM_TRY(dense_bwd_input_t<EPI_NONE>(dT1, H, PT + l.p[WT1], TIW, H, nullptr, 0, dTI, TIW, R, st));   // concat: [dOL | dLL]; FiLM: d(OL * gamma + beta)
+  LSTM_TRY(dense_bwd_input_t<EPI_NONE>(dT1, H, PT + kl.p[WT1], TIW, H, nullptr, 0, dTI, TIW, R, st));   // concat: [dOL | dLL]; FiLM: d(OL * gamma + beta)
   // gradients wrt the two latents
   const float* dOL = dTI;
   int lddOL = EL;
@@ -708,7 +721,7 @@ extern "C" int rlx_lstm_ppo_minibatch_fwdbwd_f32(const rlx_lstm_minibatch_args* 
     LSTM_LAUNCH(film_bwd_kernel, R * E, st, dTI, OL, ldOL, GB, R, E, dGB, ws + w.dOL);
     LSTM_TRY(dense_bwd_weight(LLp, L, dGB, 2 * E, L, 2 * E, R, Part, gP + l.p[WF], st));
     LSTM_TRY(colsum(dGB, 2 * E, R, 2 * E, Col, 1.f, 0.f, gP + l.p[BF], st));
-    LSTM_TRY(dense_bwd_input_t<EPI_NONE>(dGB, 2 * E, PT + l.p[WF], L, 2 * E, nullptr, 0, ws + w.dLL, L, R, st));
+    LSTM_TRY(dense_bwd_input_t<EPI_NONE>(dGB, 2 * E, PT + kl.p[WF], L, 2 * E, nullptr, 0, ws + w.dLL, L, R, st));
     dOL = ws + w.dOL; lddOL = E;
     dLL = ws + w.dLL; lddLL = L;
   }
@@ -739,7 +752,7 @@ extern "C" int rlx_lstm_ppo_minibatch_fwdbwd_f32(const rlx_lstm_minibatch_args* 
   LSTM_TRY(dense_bwd_weight(Hm, L, dG, 4 * L, L, 4 * L, R, Part, gP + l.p[WH], st));
   LSTM_TRY(colsum(dG, 4 * L, R, 4 * L, Col, 1.f, 0.f, gP + l.p[BH], st));
   LSTM_TRY(dense_bwd_weight(E1, E, dG, 4 * L, E, 4 * L, R, Part, gP + l.p[WI], st));
-  LSTM_TRY(dense_bwd_input_t<EPI_NONE>(dG, 4 * L, PT + l.p[WI], E, 4 * L, nullptr, 0, dE1, E, R, st));
+  LSTM_TRY(dense_bwd_input_t<EPI_NONE>(dG, 4 * L, PT + kl.p[WI], E, 4 * L, nullptr, 0, dE1, E, R, st));
   if (shared) LSTM_LAUNCH(cols_kernel<true>, R * E, st, dOL, lddOL, R, E, dE1, E);
   // lstm_obs_encoder backward
   LSTM_TRY(ln_param_grads(dE1, E, E1, E, Z1, E, R, E, S1, Col, gP + l.p[G1], gP + l.p[N1], st));
@@ -750,10 +763,10 @@ extern "C" int rlx_lstm_ppo_minibatch_fwdbwd_f32(const rlx_lstm_minibatch_args* 
   // ================================================================ backward: critic
   LSTM_TRY(dense_bwd_weight(C2, H, dV, 1, H, 1, R, Part, gC + l.c[WC3], st));
   LSTM_TRY(colsum(dV, 1, R, 1, Col, 1.f, 0.f, gC + l.c[BC3], st));
-  LSTM_TRY(dense_bwd_input_t<EPI_DTANH>(dV, 1, CT + l.c[WC3], H, 1, C2, H, dC2, H, R, st));
+  LSTM_TRY(dense_bwd_input_t<EPI_DTANH>(dV, 1, CT + kl.c[WC3], H, 1, C2, H, dC2, H, R, st));
   LSTM_TRY(dense_bwd_weight(C1, H, dC2, H, H, H, R, Part, gC + l.c[WC2], st));
   LSTM_TRY(colsum(dC2, H, R, H, Col, 1.f, 0.f, gC + l.c[BC2], st));
-  LSTM_TRY(dense_bwd_input_t<EPI_DTANH>(dC2, H, CT + l.c[WC2], H, H, C1, H, dC1, H, R, st));
+  LSTM_TRY(dense_bwd_input_t<EPI_DTANH>(dC2, H, CT + kl.c[WC2], H, H, C1, H, dC1, H, R, st));
   LSTM_TRY(dense_bwd_weight(X, O, dC1, H, O, H, R, Part, gC + l.c[WC1], st));
   LSTM_TRY(colsum(dC1, H, R, H, Col, 1.f, 0.f, gC + l.c[BC1], st));
   return RLX_OK;
