@@ -100,11 +100,24 @@ int rlx_pcg64_choice_i64(rlx_pcg64* st, int64_t pop_size, int64_t size, int64_t*
  * Critic: obs -> hidden -> hidden -> 1   (tanh, tanh, linear)                 ref: critic.py:23-41
  * All parameters live in ONE flat fp32 buffer; gradients and both Adam moments use the same layout.
  * Segment order (nn.Linear weights are [out, in] row-major exactly as in the reference state_dict):
- *   0 W1p[H,obs] 1 W1c[H,obs] 2 b1p[H] 3 b1c[H] 4 W2p[H,H] 5 W2c[H,H] 6 b2p[H] 7 b2c[H]
+ *   0 W1p[H,P]   1 W1c[H,C]  2 b1p[H] 3 b1c[H] 4 W2p[H,H] 5 W2c[H,H] 6 b2p[H] 7 b2c[H]
  *   8 W3p[A,H]   9 W3c[1,H]  10 b3p[A] 11 b3c[1] 12 logstd[A]
- * (policy and critic first layers are adjacent so that layer 1 runs as one [2H, obs] GEMM on the shared input.) */
+ * (policy and critic first layers are adjacent so that layer 1 runs as one [2H, obs] GEMM on the shared input.)
+ *
+ * Observation index sets (the env's policy_observation_indices / critic_observation_indices; ref: policy.py:14,36-37,62,
+ * critic.py:10,26-27,45): the policy reads x[:, policy_idx] (P = policy_in_dim columns), the critic x[:, critic_idx] (C columns).
+ * policy_idx / critic_idx are DEVICE int32 arrays of distinct indices in [0, obs_dim); the caller validates them (the library cannot
+ * read device memory before it launches).  NULL = identity with in_dim 0 or obs_dim; a non-NULL array needs 1 <= in_dim <= obs_dim.
+ * With an array present every call that reads layer 1 first embeds W1p / W1c into a zero-filled [2H, obs] workspace matrix
+ * (W1cat[h, policy_idx[j]] = W1p[h, j], W1cat[H + h, critic_idx[j]] = W1c[h, j]) and runs the full-width GEMMs on it; the [2H, obs]
+ * layer-1 gradient is folded back onto the selected columns.  A zero-initialised tail means obs_dim inputs for both nets. */
 #define RLX_PPO_NSEG 13
-typedef struct rlx_ppo_dims { int32_t obs_dim, act_dim, hidden; } rlx_ppo_dims;
+typedef struct rlx_ppo_dims {
+  int32_t obs_dim, act_dim, hidden;
+  int32_t policy_in_dim, critic_in_dim;  /* P, C; 0 = obs_dim */
+  const int32_t* policy_idx;             /* [P] device array, or NULL = identity */
+  const int32_t* critic_idx;             /* [C] device array, or NULL = identity */
+} rlx_ppo_dims;
 int64_t rlx_ppo_param_count(const rlx_ppo_dims* d);
 /* offsets[RLX_PPO_NSEG+1]: start of each segment, last entry = total count.  is_critic[RLX_PPO_NSEG]: 0 policy / 1 critic. */
 int rlx_ppo_param_layout(const rlx_ppo_dims* d, int64_t* offsets, int32_t* is_critic);

@@ -15,7 +15,9 @@ c_float_p = C.c_void_p  # raw device / host addresses are passed as integers
 
 
 class PpoDims(C.Structure):
-    _fields_ = [("obs_dim", C.c_int32), ("act_dim", C.c_int32), ("hidden", C.c_int32)]
+    """rlx_ppo_dims.  The tail (observation index sets) defaults to zeros / NULL: both nets read every observation column."""
+    _fields_ = [("obs_dim", C.c_int32), ("act_dim", C.c_int32), ("hidden", C.c_int32), ("policy_in_dim", C.c_int32),
+                ("critic_in_dim", C.c_int32), ("policy_idx", C.c_void_p), ("critic_idx", C.c_void_p)]
 
 
 class Pcg64(C.Structure):
@@ -390,19 +392,50 @@ class Pcg64Generator:
 SEGMENT_NAMES = ("W1p", "W1c", "b1p", "b1c", "W2p", "W2c", "b2p", "b2c", "W3p", "W3c", "b3p", "b3c", "logstd")
 
 
-def ppo_layout(obs_dim, act_dim, hidden):
+def ppo_layout(obs_dim, act_dim, hidden, dims=None):
+    """dims: a PpoDims carrying observation index sets (overrides the three sizes)."""
     lib = load()
-    d = PpoDims(obs_dim, act_dim, hidden)
+    d = PpoDims(obs_dim, act_dim, hidden) if dims is None else dims
     off = (C.c_int64 * (RLX_PPO_NSEG + 1))()
     crit = (C.c_int32 * RLX_PPO_NSEG)()
     check(lib.rlx_ppo_param_layout(C.byref(d), off, crit), "ppo_param_layout")
     return list(off), list(crit)
 
 
-def segment_shapes(obs_dim, act_dim, hidden):
+def segment_shapes(obs_dim, act_dim, hidden, policy_in_dim=None, critic_in_dim=None):
+    """Reference shapes of the segments; policy_in_dim / critic_in_dim: lengths of the observation index sets (None = obs_dim)."""
     H, O, A = hidden, obs_dim, act_dim
-    return {"W1p": (H, O), "W1c": (H, O), "b1p": (H,), "b1c": (H,), "W2p": (H, H), "W2c": (H, H), "b2p": (H,), "b2c": (H,),
+    P = O if policy_in_dim is None else int(policy_in_dim)
+    Cc = O if critic_in_dim is None else int(critic_in_dim)
+    return {"W1p": (H, P), "W1c": (H, Cc), "b1p": (H,), "b1c": (H,), "W2p": (H, H), "W2c": (H, H), "b2p": (H,), "b2c": (H,),
             "W3p": (A, H), "W3c": (1, H), "b3p": (A,), "b3c": (1,), "logstd": (1, A)}
+
+
+def observation_indices(name, ind, obs_dim):
+    """The env attribute `name` (policy_observation_indices / critic_observation_indices) as an int64 numpy array, or None when it is
+    absent or the identity.  Refuses, with ValueError, anything that is not a non-empty 1-D integer array of distinct indices in
+    [0, obs_dim): duplicates because in bf16-autocast mode the two separately rounded weights of a repeated column would be summed into
+    one operand that is not a bf16 value (the reference multiplies each copy by its own bf16 weight)."""
+    if ind is None:
+        return None
+    if hasattr(ind, "detach"):  # torch tensor
+        ind = ind.detach().cpu().numpy()
+    a = np.asarray(ind)
+    if a.ndim != 1:
+        raise ValueError(f"{name} must be a 1-D array of observation indices, got shape {a.shape}")
+    if a.size == 0:
+        raise ValueError(f"{name} must not be empty")
+    if a.dtype == np.bool_ or not np.issubdtype(a.dtype, np.integer):
+        raise ValueError(f"{name} must hold integers, got dtype {a.dtype}")
+    a = a.astype(np.int64)
+    if a.min() < 0 or a.max() >= obs_dim:
+        raise ValueError(f"{name} must lie in [0, {obs_dim}), got values in [{a.min()}, {a.max()}]")
+    if np.unique(a).size != a.size:
+        raise ValueError(f"{name} holds duplicate indices: not supported (in bf16-autocast mode a repeated column's two bf16 weights "
+                         f"would be summed into one operand that is no longer a bf16 value)")
+    if a.size == obs_dim and np.array_equal(a, np.arange(obs_dim)):
+        return None
+    return a
 
 
 # reference state_dict key <-> segment (policy.py:45-52, critic.py:29-35)

@@ -29,17 +29,36 @@ def _stream():
 
 
 class PpoKernels:
-    """Binds the library for one (obs_dim, act_dim, hidden) network shape."""
+    """Binds the library for one (obs_dim, act_dim, hidden) network shape.
 
-    def __init__(self, obs_dim, act_dim, hidden):
+    policy_idx / critic_idx: the observation columns each net reads (the env's policy_observation_indices / critic_observation_indices),
+    validated by the caller (nt.observation_indices), or None = every column.  They are passed to the library as int32 device arrays
+    owned by this object, exactly as given: an explicit arange(obs_dim) takes the embedded layer-1 path."""
+
+    def __init__(self, obs_dim, act_dim, hidden, policy_idx=None, critic_idx=None, device=None):
         self.lib = nt.load()
         self.dims = nt.PpoDims(int(obs_dim), int(act_dim), int(hidden))
         self.obs_dim, self.act_dim, self.hidden = int(obs_dim), int(act_dim), int(hidden)
+        self.policy_in_dim = self.critic_in_dim = self.obs_dim
+        self.policy_idx_dev = self.critic_idx_dev = None
+        if policy_idx is not None or critic_idx is not None:
+            device = torch.device("cuda", torch.cuda.current_device()) if device is None else device
+            if policy_idx is not None:
+                self.policy_idx_dev = torch.as_tensor(np.asarray(policy_idx), dtype=torch.int32).contiguous().to(device)
+                self.policy_in_dim = int(self.policy_idx_dev.numel())
+                self.dims.policy_in_dim, self.dims.policy_idx = self.policy_in_dim, self.policy_idx_dev.data_ptr()
+            if critic_idx is not None:
+                self.critic_idx_dev = torch.as_tensor(np.asarray(critic_idx), dtype=torch.int32).contiguous().to(device)
+                self.critic_in_dim = int(self.critic_idx_dev.numel())
+                self.dims.critic_in_dim, self.dims.critic_idx = self.critic_in_dim, self.critic_idx_dev.data_ptr()
         n = self.lib.rlx_ppo_param_count(C.byref(self.dims))
         if n <= 0:
             raise RuntimeError(f"rl_x_b200: unsupported network shape obs={obs_dim} act={act_dim} hidden={hidden}: {nt.last_error()}")
         self.param_count = int(n)
-        self.offsets, self.is_critic = nt.ppo_layout(obs_dim, act_dim, hidden)
+        self.offsets, self.is_critic = nt.ppo_layout(obs_dim, act_dim, hidden, self.dims)
+
+    def segment_shapes(self):
+        return nt.segment_shapes(self.obs_dim, self.act_dim, self.hidden, self.policy_in_dim, self.critic_in_dim)
 
     # ---------------------------------------------------------------------------------------------- workspaces
     def forward_workspace(self, n, device):

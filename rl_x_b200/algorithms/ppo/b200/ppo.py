@@ -35,11 +35,14 @@ from rl_x_b200.environments.types import DataInterfaceType, same_member
 rlx_logger = logging.getLogger("rl_x")
 
 
-def init_reference_parameters(obs_dim, act_dim, hidden, std_dev, seed):
+def init_reference_parameters(obs_dim, act_dim, hidden, std_dev, seed, policy_in_dim=None, critic_in_dim=None):
     """Initial weights bit-identical to the reference for the same seed: torch.manual_seed(seed) (ppo.py:73), then the
     policy's three nn.Linear layers (constructor init followed by orthogonal_/constant_, policy.py:45-58) and the critic's
-    (critic.py:29-41), created on the CPU in that order.  Returns {reference state_dict key: tensor}."""
+    (critic.py:29-41), created on the CPU in that order.  policy_in_dim / critic_in_dim: lengths of the env's observation index
+    sets (the first layers' inputs, policy.py:37, critic.py:27; None = obs_dim).  Returns {reference state_dict key: tensor}."""
     torch.manual_seed(seed)
+    p_in = obs_dim if policy_in_dim is None else int(policy_in_dim)
+    c_in = obs_dim if critic_in_dim is None else int(critic_in_dim)
 
     def layer(i, o, std):
         lin = nn.Linear(i, o)
@@ -48,11 +51,11 @@ def init_reference_parameters(obs_dim, act_dim, hidden, std_dev, seed):
         return lin
 
     out = {}
-    pol = [layer(obs_dim, hidden, np.sqrt(2)), layer(hidden, hidden, np.sqrt(2)), layer(hidden, act_dim, 0.01)]
+    pol = [layer(p_in, hidden, np.sqrt(2)), layer(hidden, hidden, np.sqrt(2)), layer(hidden, act_dim, 0.01)]
     for idx, lin in zip((0, 2, 4), pol):
         out[f"policy_mean.{idx}.weight"], out[f"policy_mean.{idx}.bias"] = lin.weight.detach().clone(), lin.bias.detach().clone()
     out["policy_logstd"] = torch.full((1, act_dim), np.log(std_dev).item())
-    cri = [layer(obs_dim, hidden, np.sqrt(2)), layer(hidden, hidden, np.sqrt(2)), layer(hidden, 1, 1.0)]
+    cri = [layer(c_in, hidden, np.sqrt(2)), layer(hidden, hidden, np.sqrt(2)), layer(hidden, 1, 1.0)]
     for idx, lin in zip((0, 2, 4), cri):
         out[f"critic.{idx}.weight"], out[f"critic.{idx}.bias"] = lin.weight.detach().clone(), lin.bias.detach().clone()
     return out
@@ -76,7 +79,7 @@ class FlatParameters:
     def __init__(self, kernels, device):
         self.k = kernels
         self.flat = torch.zeros(kernels.param_count, dtype=torch.float32, device=device)
-        self.shapes = nt.segment_shapes(kernels.obs_dim, kernels.act_dim, kernels.hidden)
+        self.shapes = kernels.segment_shapes()
 
     def view(self, flat, seg):
         i = nt.SEGMENT_NAMES.index(seg)
@@ -239,6 +242,15 @@ class PPO:
         self.bf16_mixed_precision_training = bool(config.algorithm.get("bf16_mixed_precision_training", False))
         if self.bf16_mixed_precision_training and self.world_size > 1:
             raise NotImplementedError("rl_x_b200 PPO: bf16_mixed_precision_training is single-GPU in this build.")
+        # the columns each net reads (policy.py:14,36-37,62, critic.py:10,26-27,45), validated on the host before any device work;
+        # None = all of them, in order
+        self.policy_observation_indices = self.critic_observation_indices = None
+        os_shape = self.train_env.single_observation_space.shape
+        if len(os_shape) == 1:
+            self.policy_observation_indices = nt.observation_indices(
+                "policy_observation_indices", getattr(self.train_env, "policy_observation_indices", None), int(os_shape[0]))
+            self.critic_observation_indices = nt.observation_indices(
+                "critic_observation_indices", getattr(self.train_env, "critic_observation_indices", None), int(os_shape[0]))
         if config.algorithm.device != "gpu" or not torch.cuda.is_available():
             raise RuntimeError("rl_x_b200 PPO needs a CUDA device (algorithm.device=gpu); there is no CPU fallback.")
         self.device = torch.device("cuda", torch.cuda.current_device())
@@ -258,17 +270,15 @@ class PPO:
         if len(self.os_shape) != 1 or len(self.as_shape) != 1:
             raise ValueError("rl_x_b200 PPO supports flat observations and flat continuous actions only.")
         obs_dim, act_dim = int(self.os_shape[0]), int(self.as_shape[0])
-        for attr in ("policy_observation_indices", "critic_observation_indices"):
-            ind = getattr(self.train_env, attr, None)
-            if ind is not None and not np.array_equal(np.asarray(ind), np.arange(obs_dim)):
-                raise ValueError(f"rl_x_b200 PPO does not implement a non-identity {attr} (policy.py:14, critic.py:10).")
 
-        self.kernels = PpoKernels(obs_dim, act_dim, self.nr_hidden_units)
+        self.kernels = PpoKernels(obs_dim, act_dim, self.nr_hidden_units, self.policy_observation_indices, self.critic_observation_indices,
+                                  self.device)
         engine = config.algorithm.get("gemm_engine", "auto")
         lib = self.kernels.lib
         lib.rlx_set_gemm_engine({"simt": 0, "tcgen05": 1, "auto": 1}[engine])
         self.params = FlatParameters(self.kernels, self.device)
-        self.params.load_named(init_reference_parameters(obs_dim, act_dim, self.nr_hidden_units, self.std_dev, self.model_seed))
+        self.params.load_named(init_reference_parameters(obs_dim, act_dim, self.nr_hidden_units, self.std_dev, self.model_seed,
+                                                         self.kernels.policy_in_dim, self.kernels.critic_in_dim))
         if self.dist:
             self.dist.broadcast(self.params.flat, src=0)  # bit-identical replicas even if a rank's torch build initialises differently
         P = self.kernels.param_count

@@ -131,14 +131,25 @@ __device__ __forceinline__ float block_sum(float v, float* sh) {
 struct PpoLayout {
   int64_t off[RLX_PPO_NSEG + 1];
   int obs, act, H;
+  int in_p, in_c;                 // layer-1 inputs of the policy / critic (= obs without index sets)
+  const int32_t* pidx;            // observation index sets (device), null = identity
+  const int32_t* cidx;
+  bool embed;                     // an index set is present: layer 1 runs on the embedded [2H, obs] matrix
   __host__ __device__ int64_t total() const { return off[RLX_PPO_NSEG]; }
 };
 enum Seg { W1P = 0, W1C, B1P, B1C, W2P, W2C, B2P, B2C, W3P, W3C, B3P, B3C, LOGSTD };
 
+inline int ppo_in_dim(int32_t in_dim, int32_t obs) { return in_dim > 0 ? in_dim : obs; }
+
 inline PpoLayout make_layout(const rlx_ppo_dims& d) {
   PpoLayout L;
-  const int64_t H = d.hidden, O = d.obs_dim, A = d.act_dim;
-  const int64_t sz[RLX_PPO_NSEG] = {H * O, H * O, H, H, H * H, H * H, H, H, A * H, H, A, 1, A};
+  const int64_t H = d.hidden, A = d.act_dim;
+  L.in_p = ppo_in_dim(d.policy_in_dim, d.obs_dim);
+  L.in_c = ppo_in_dim(d.critic_in_dim, d.obs_dim);
+  L.pidx = d.policy_idx;
+  L.cidx = d.critic_idx;
+  L.embed = d.policy_idx != nullptr || d.critic_idx != nullptr;
+  const int64_t sz[RLX_PPO_NSEG] = {H * L.in_p, H * L.in_c, H, H, H * H, H * H, H, H, A * H, H, A, 1, A};
   int64_t o = 0;
   for (int i = 0; i < RLX_PPO_NSEG; ++i) {
     L.off[i] = o;
@@ -172,8 +183,24 @@ __device__ __forceinline__ int net_of(const PpoNetMap& map, long long i) {
   return (map.critic_mask >> seg) & 1u;
 }
 
+// What is wrong with the observation index fields of d (include/rlx_b200.h), or null.  The index VALUES live on the device and are
+// the caller's to validate.
+inline const char* ppo_index_problem(const rlx_ppo_dims& d) {
+  const int32_t in[2] = {d.policy_in_dim, d.critic_in_dim};
+  const int32_t* idx[2] = {d.policy_idx, d.critic_idx};
+  for (int k = 0; k < 2; ++k) {
+    if (idx[k] != nullptr && (in[k] < 1 || in[k] > d.obs_dim))
+      return k == 0 ? "policy_idx given: policy_in_dim must be in [1, obs_dim]" : "critic_idx given: critic_in_dim must be in [1, obs_dim]";
+    if (idx[k] == nullptr && in[k] != 0 && in[k] != d.obs_dim)
+      return k == 0 ? "policy_idx is NULL (identity): policy_in_dim must be 0 or obs_dim"
+                    : "critic_idx is NULL (identity): critic_in_dim must be 0 or obs_dim";
+  }
+  return nullptr;
+}
+
 inline bool dims_ok(const rlx_ppo_dims& d) {
-  return d.obs_dim > 0 && d.act_dim > 0 && d.hidden > 0 && d.act_dim <= 64 && d.hidden <= 4096 && d.obs_dim <= 65536;
+  return d.obs_dim > 0 && d.act_dim > 0 && d.hidden > 0 && d.act_dim <= 64 && d.hidden <= 4096 && d.obs_dim <= 65536 &&
+         ppo_index_problem(d) == nullptr;
 }
 
 }  // namespace rlx

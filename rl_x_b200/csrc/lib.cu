@@ -77,14 +77,18 @@ extern "C" int rlx_set_autocast_bf16(int on) {
 
 extern "C" int64_t rlx_ppo_param_count(const rlx_ppo_dims* d) {
   if (d == nullptr || !rlx::dims_ok(*d)) {
-    rlx::set_error("rlx_ppo_param_count: unsupported dims");
+    const char* ip = d ? rlx::ppo_index_problem(*d) : nullptr;
+    rlx::set_error("rlx_ppo_param_count: %s", ip ? ip : "unsupported dims");
     return RLX_ERR_INVALID_ARG;
   }
   return rlx::make_layout(*d).total();
 }
 
 extern "C" int rlx_ppo_param_layout(const rlx_ppo_dims* d, int64_t* offsets, int32_t* is_critic) {
-  RLX_CHECK_ARG(d != nullptr && rlx::dims_ok(*d), "unsupported dims");
+  RLX_CHECK_ARG(d != nullptr, "dims is null");
+  const char* ip = rlx::ppo_index_problem(*d);
+  RLX_CHECK_ARG(ip == nullptr, ip);
+  RLX_CHECK_ARG(rlx::dims_ok(*d), "unsupported dims");
   RLX_CHECK_ARG(offsets != nullptr, "offsets is null");
   const rlx::PpoLayout L = rlx::make_layout(*d);
   for (int i = 0; i <= RLX_PPO_NSEG; ++i) offsets[i] = L.off[i];

@@ -81,8 +81,43 @@ static int round_inputs_bf16(const PpoLayout& L, const float*& params, const flo
   return RLX_OK;
 }
 
+// Observation index sets: the layer-1 operand W1cat [2H, obs] = zeros, with W1p [H, P] scattered into the policy_idx columns of rows
+// 0..H-1 and W1c [H, C] into the critic_idx columns of rows H..2H-1.  For distinct indices every product the reference's index-select
+// forms is formed once and the rest are x * 0, so the GEMMs, the tf32 split, the bf16 rounding and the dW1 | db1 GEMM run unchanged at
+// the full observation width.  One CTA per row: zero it, then scatter (the barrier orders the two stores).
+__global__ void __launch_bounds__(256) ppo_embed_w1_kernel(const float* __restrict__ w1p, const float* __restrict__ w1c, const int32_t* __restrict__ pidx,
+                                                           const int32_t* __restrict__ cidx, int H, int obs, int in_p, int in_c, float* __restrict__ out) {
+  const int row = blockIdx.x;
+  float* dst = out + (long long)row * obs;
+  for (int c = threadIdx.x; c < obs; c += blockDim.x) dst[c] = 0.f;
+  __syncthreads();
+  const bool critic = row >= H;
+  const int in = critic ? in_c : in_p;
+  const int32_t* idx = critic ? cidx : pidx;
+  const float* src = critic ? w1c + (long long)(row - H) * in_c : w1p + (long long)row * in_p;
+  for (int j = threadIdx.x; j < in; j += blockDim.x) dst[idx ? idx[j] : j] = src[j];
+}
+
+// The layer-1 weight operand [2H, obs] of this call: W1p | W1c of `params` in place, or (index sets) the embedded matrix written into
+// `emb` from the current parameters - on every call, so that whatever wrote them last is what the GEMMs see
+static int layer1_weights(const PpoLayout& L, const float* params, float* emb, const float*& w1, cudaStream_t st) {
+  if (!L.embed) {
+    w1 = params + L.off[W1P];
+    return RLX_OK;
+  }
+  const double bytes = 4.0 * L.H * (2.0 * L.obs + 2.0 * L.in_p + 2.0 * L.in_c);
+  RLX_LAUNCH_C(KC_OTHER, 0, bytes, ppo_embed_w1_kernel, (unsigned)(2 * L.H), 256, 0, st, params + L.off[W1P], params + L.off[W1C], L.pidx, L.cidx,
+               L.H, L.obs, L.in_p, L.in_c, emb);
+  w1 = emb;
+  return RLX_OK;
+}
+// workspace floats of the embedded matrix (none without index sets)
+static size_t embed_floats(const rlx_ppo_dims& d) {
+  return make_layout(d).embed ? (size_t)2 * d.hidden * d.obs_dim : 0;
+}
+
 struct FwdPlan {
-  size_t off_H1, off_H2, off_P, off_X, total;
+  size_t off_H1, off_H2, off_P, off_X, off_W1, total;
 };
 static FwdPlan plan_forward(const rlx_ppo_dims& d, long long n) {
   FwdPlan P;
@@ -93,6 +128,7 @@ static FwdPlan plan_forward(const rlx_ppo_dims& d, long long n) {
   // bf16-autocast mode: rounded copies of the parameters and of the observations (always planned: the mode is a run-time switch)
   P.off_P = o; o += align_up((size_t)make_layout(d).total() * sizeof(float), 256);
   P.off_X = o; o += align_up((size_t)n * d.obs_dim * sizeof(float), 256);
+  P.off_W1 = o; o += align_up(embed_floats(d) * sizeof(float), 256);  // observation index sets: embedded layer-1 matrix
   P.total = o;
   return P;
 }
@@ -103,7 +139,8 @@ constexpr int kHeadWgradRows = 64;
 enum { WS_W1_HI, WS_W1_LO, WS_W2_HI, WS_W2_LO, WS_W2T_HI, WS_W2T_LO, WS_COUNT };
 
 struct TrainPlan {
-  size_t off_H1, off_H2, off_dZ2, off_dZ1, off_dhead, off_headpart, off_part1, off_rs1, off_part2, off_part3, off_norm, off_barrier, off_P, off_X, off_ratio, total;
+  size_t off_H1, off_H2, off_dZ2, off_dZ1, off_dhead, off_headpart, off_part1, off_rs1, off_part2, off_part3, off_norm, off_barrier, off_P, off_X, off_ratio,
+      off_W1, total;
   size_t off_wsplit[WS_COUNT];
   int max_s1, max_s2, max_s3;
   int head_blocks, wgrad_chunks, norm_blocks, head_npart;
@@ -145,6 +182,7 @@ static TrainPlan plan_train(const rlx_ppo_dims& d, long long m) {
   take(P.off_X, (size_t)m * (size_t)(ceil_div(O + 1, 4) * 4));             // ... and rounded copy of the minibatch states (pitch <= obs + 4)
   take(P.off_ratio, (size_t)m);                                           // ESPO median: |ratio - 1| per row
   for (int i = 0; i < WS_COUNT; ++i) take(P.off_wsplit[i], i < WS_W2_HI ? (size_t)(2 * H * O) : (size_t)(2 * H * H));
+  take(P.off_W1, embed_floats(d));                                        // observation index sets: embedded layer-1 matrix
   P.total = o;
   return P;
 }
@@ -164,24 +202,24 @@ static size_t head_smem_bytes(const rlx_ppo_dims& d, bool train) {
 struct SplitWeights {
   const float* p[WS_COUNT];
 };
-static int split_weights(const PpoLayout& L, const float* params, void* ws, const TrainPlan& P, SplitWeights& sw, cudaStream_t st) {
+static int split_weights(const PpoLayout& L, const float* params, const float* w1, void* ws, const TrainPlan& P, SplitWeights& sw, cudaStream_t st) {
   const int H = L.H;
   float* w[WS_COUNT];
   for (int i = 0; i < WS_COUNT; ++i) sw.p[i] = w[i] = ws_ptr<float>(ws, P.off_wsplit[i]);
-  const Tf32SplitJob jobs[3] = {{params + L.off[W1P], w[WS_W1_HI], w[WS_W1_LO], 1, 2 * H, L.obs, 0},
+  const Tf32SplitJob jobs[3] = {{w1, w[WS_W1_HI], w[WS_W1_LO], 1, 2 * H, L.obs, 0},
                                 {params + L.off[W2P], w[WS_W2_HI], w[WS_W2_LO], 1, 2 * H, H, 0},
                                 {params + L.off[W2P], w[WS_W2T_HI], w[WS_W2T_LO], 2, H, H, 1}};
   return tf32_split(jobs, 3, KC_GEMM_FWD, st);  // a few microseconds, charged to the forward GEMMs
 }
 
-// hidden layers: H1 = tanh(X W1cat^T + b1cat), H2 = tanh(H1 (blockdiag W2)^T + b2cat).  ldx = row pitch of X.  sw: tf32 hi / lo copies of
-// W1cat and W2 (wgmma engine, fp32 mode), or null.
-static int mlp_hidden_forward(const rlx_ppo_dims& d, const PpoLayout& L, const float* params, const float* X, long long ldx, long long rows,
-                              float* H1, float* H2, cudaStream_t stream, int bf16 = 0, const SplitWeights* sw = nullptr) {
+// hidden layers: H1 = tanh(X W1cat^T + b1cat), H2 = tanh(H1 (blockdiag W2)^T + b2cat).  w1 = W1cat [2H, obs] (layer1_weights).  ldx = row
+// pitch of X.  sw: tf32 hi / lo copies of W1cat and W2 (wgmma engine, fp32 mode), or null.
+static int mlp_hidden_forward(const rlx_ppo_dims& d, const PpoLayout& L, const float* params, const float* w1, const float* X, long long ldx,
+                              long long rows, float* H1, float* H2, cudaStream_t stream, int bf16 = 0, const SplitWeights* sw = nullptr) {
   const int H = L.H;
   const bool tc = use_tc(d);
   GemmP g{};
-  g.A = X; g.B = params + L.off[W1P]; g.C = H1; g.bias = params + L.off[B1P];
+  g.A = X; g.B = w1; g.C = H1; g.bias = params + L.off[B1P];
   g.M = (int)rows; g.N = 2 * H; g.K = L.obs;
   g.lda = (int)ldx; g.ldb = L.obs; g.ldc = 2 * H;
   g.splits = 1; g.kchunk = (int)(ceil_div(L.obs, 8) * 8);
@@ -248,6 +286,8 @@ extern "C" size_t rlx_ppo_forward_workspace_bytes(const rlx_ppo_dims* d, int64_t
 
 extern "C" int rlx_ppo_forward_f32(const rlx_ppo_forward_args* a, void* stream) {
   RLX_CHECK_ARG(a != nullptr, "args is null");
+  const char* ip = ppo_index_problem(a->dims);
+  RLX_CHECK_ARG(ip == nullptr, ip);
   RLX_CHECK_ARG(head_dims_ok(a->dims), "unsupported dims (act <= 64, hidden <= 1024)");
   RLX_CHECK_ARG(a->n >= 0 && a->n < (1LL << 31), "bad row count");
   if (a->n == 0) return RLX_OK;
@@ -270,7 +310,10 @@ extern "C" int rlx_ppo_forward_f32(const rlx_ppo_forward_args* a, void* stream) 
     rc = round_inputs_bf16(L, params, obs, a->n * (long long)L.obs, ws_ptr<float>(a->workspace, P.off_P), ws_ptr<float>(a->workspace, P.off_X), st);
     if (rc) return rc;
   }
-  rc = mlp_hidden_forward(a->dims, L, params, obs, a->dims.obs_dim, a->n, H1, H2, st, bf16);
+  const float* w1 = nullptr;
+  rc = layer1_weights(L, params, ws_ptr<float>(a->workspace, P.off_W1), w1, st);
+  if (rc) return rc;
+  rc = mlp_hidden_forward(a->dims, L, params, w1, obs, a->dims.obs_dim, a->n, H1, H2, st, bf16);
   if (rc) return rc;
   HeadP h{};
   fill_head_common(h, L, params, H2, a->n);
@@ -302,6 +345,8 @@ extern "C" size_t rlx_ppo_minibatch_workspace_bytes(const rlx_ppo_dims* d, int64
 
 static int check_mb_args(const rlx_ppo_minibatch_args* a, bool need_data, TrainPlan& P) {
   RLX_CHECK_ARG(a != nullptr, "args is null");
+  const char* ip = ppo_index_problem(a->dims);
+  RLX_CHECK_ARG(ip == nullptr, ip);
   RLX_CHECK_ARG(head_dims_ok(a->dims), "unsupported dims (act <= 64, hidden <= 1024)");
   RLX_CHECK_ARG(a->m >= 0 && a->m < (1LL << 31) && a->m_global >= 1, "bad minibatch size");
   RLX_CHECK_ARG(a->params && a->grads, "params / grads is null");
@@ -599,6 +644,12 @@ static GradReduceP make_grad_reduce(const rlx_ppo_minibatch_args* a, const PpoLa
   const float inv_mg = 1.f / (float)a->m_global;
   GradReduceP r{};
   r.g[0] = GradGroup{L.off[W1P], 2LL * H * O, ws_ptr<float>(ws, P.off_part1), s1, 2LL * H * O};
+  if (L.embed) {
+    // the dW1 partials are [2H, obs] gradients of the embedded matrix: fold them onto W1p [H, P] | W1c [H, C]
+    r.g[0].len = (long long)H * (L.in_p + L.in_c);
+    r.g[0].map0 = L.pidx; r.g[0].map1 = L.cidx;
+    r.g[0].in0 = L.in_p; r.g[0].in1 = L.in_c; r.g[0].rows = H; r.g[0].ld = O;
+  }
   r.g[1] = GradGroup{L.off[B1P], 2LL * H, ws_ptr<float>(ws, P.off_rs1), s1, 2LL * H};
   r.g[2] = GradGroup{L.off[W2P], 2LL * H * H, ws_ptr<float>(ws, P.off_part2), s2, 2LL * H * H};
   r.g[3] = GradGroup{L.off[B2P], 2LL * H, headpart + (2 * A + 5), head_blocks, (long long)npart};
@@ -651,13 +702,16 @@ static int minibatch_fwdbwd(const rlx_ppo_minibatch_args* a, void* stream, bool 
     }
     // wgmma engine, fp32: split the weights once here rather than in every tile of the forward and dX GEMMs.  Made from the current
     // parameters on every call, so whatever wrote them last (Adam, init, a checkpoint load, a broadcast) is what the GEMMs see.
+    const float* w1 = nullptr;
+    rc = layer1_weights(L, params, ws_ptr<float>(ws, P.off_W1), w1, st);
+    if (rc) return rc;
     SplitWeights sw{};
     const bool presplit = tc && !bf16;
     if (presplit) {
-      rc = split_weights(L, params, ws, P, sw, st);
+      rc = split_weights(L, params, w1, ws, P, sw, st);
       if (rc) return rc;
     }
-    rc = mlp_hidden_forward(a->dims, L, params, states, ldx, m, ws_ptr<float>(ws, P.off_H1), ws_ptr<float>(ws, P.off_H2), st, bf16,
+    rc = mlp_hidden_forward(a->dims, L, params, w1, states, ldx, m, ws_ptr<float>(ws, P.off_H1), ws_ptr<float>(ws, P.off_H2), st, bf16,
                             presplit ? &sw : nullptr);
     if (rc) return rc;
     head_blocks = launch_train_head(a, L, P, params, bf16, st);

@@ -13,8 +13,28 @@ struct GradGroup {
   const float* src;        // partials: element i of split s at src[s*stride + i]
   int nsplit;
   long long stride;
+  // Optional column map (layer 1 with observation index sets; ld == 0 = off): the flat range holds part 0 [rows, in0] then part 1
+  // [rows, in1] (policy, critic weights), and element (r, j) of part k reads the partials at ((k * rows + r) * ld + map_k[j]) - the
+  // [2H, obs] gradient of the embedded layer-1 matrix folded back onto the selected columns (null map_k = identity).  Columns no net
+  // selected are dropped.
+  const int32_t* map0;
+  const int32_t* map1;
+  int in0, in1, rows, ld;
 };
 constexpr int kNumGroups = 7;
+
+// offset into a split's partials of element e of group g
+__device__ __forceinline__ long long grad_src_index(const GradGroup& g, long long e) {
+  if (g.ld == 0) return e;
+  const long long len0 = (long long)g.rows * g.in0;
+  const int part = e >= len0 ? 1 : 0;
+  if (part) e -= len0;
+  const int in = part ? g.in1 : g.in0;
+  const long long r = e / in;
+  const int j = (int)(e - r * in);
+  const int32_t* map = part ? g.map1 : g.map0;
+  return ((long long)part * g.rows + r) * g.ld + (map ? map[j] : j);
+}
 
 struct GradReduceP {
   GradGroup g[kNumGroups];
@@ -78,7 +98,7 @@ __global__ void __launch_bounds__(256) ppo_grad_reduce_kernel(const GradReduceP 
         const GradGroup& g = p.g[gi];
         if (i >= g.off && i < g.off + g.len) {
           if (g.nsplit > kTallSplit) mine = false;
-          else s = grad_sum_serial(g.src + (i - g.off), g.nsplit, g.stride);
+          else s = grad_sum_serial(g.src + grad_src_index(g, i - g.off), g.nsplit, g.stride);
         }
       }
       if (mine) {
@@ -97,7 +117,7 @@ __global__ void __launch_bounds__(256) ppo_grad_reduce_kernel(const GradReduceP 
       const GradGroup& g = p.g[gi];
       if (g.nsplit <= kTallSplit) continue;
       if (w >= 0 && w < g.len) {
-        float s = grad_sum_warp(g.src + w, g.nsplit, g.stride, lane);
+        float s = grad_sum_warp(g.src + grad_src_index(g, w), g.nsplit, g.stride, lane);
         const long long i = g.off + w;
         if (i >= p.logstd_off && i < p.logstd_off + p.act) s += p.entropy_grad;
         else s = bf16r_if(s, p.bf16);
