@@ -584,7 +584,7 @@ typedef struct rlx_sac_update_args {
   rlx_sac_dims dims;
   int64_t batch;
   float* policy;            /* [Pp] */
-  float* q;                 /* [4][Pq] */
+  float* q;                 /* [4][Pq]; each net's pad must hold finite values (zeros): the tensor engine reads it as the K tail of a weight */
   float* log_alpha;         /* [1] */
   const float* states;      /* [batch, obs]   sampled batch (rlx_replay_sample_gather_f32) */
   const float* next_states; /* [batch, obs] */
@@ -598,7 +598,7 @@ typedef struct rlx_sac_update_args {
   float gamma, tau, target_entropy;
   float adam_beta1, adam_beta2, adam_eps;
   float* g_policy; float* m_policy; float* v_policy;            /* [Pp] each */
-  float* g_q; float* m_q; float* v_q;                           /* [2*Pq] each (online nets) */
+  float* g_q; float* m_q; float* v_q;                           /* [2*Pq] each (online nets); g_q's per-net pad is written 0 */
   float* g_log_alpha; float* m_log_alpha; float* v_log_alpha;   /* [1] each */
   const float* lr;          /* [1] device */
   int64_t* steps;           /* [3] device: Adam step counters of policy, q, log_alpha */

@@ -68,12 +68,16 @@ class Learner:
     """ref: SAC.__init__ optimisers (sac.py:74-77) and one iteration of the optimisation block (sac.py:219-259)."""
 
     def __init__(self, pol, q1, q2, low, high, lr=3e-4, gamma=0.99, tau=0.005, target_entropy=None, ls_min=-20.0, ls_max=2.0, log_alpha=0.0,
-                 q1_target=None, q2_target=None):
-        g = lambda d: {k: v.clone().requires_grad_(True) for k, v in d.items()}
+                 q1_target=None, q2_target=None, dtype=torch.float32, device="cpu"):
+        """dtype / device: where the learner's parameters, log_alpha and action bounds live (the caller's batches must match).  The float32
+        CPU default is the pinned oracle; float64 is the high-precision reference of the GPU tests."""
+        to = lambda v: v.to(device, dtype).clone()
+        g = lambda d: {k: to(v).requires_grad_(True) for k, v in d.items()}
         self.pol, self.q1, self.q2 = g(pol), g(q1), g(q2)
-        self.q1t = {k: v.clone() for k, v in (q1_target or q1).items()}
-        self.q2t = {k: v.clone() for k, v in (q2_target or q2).items()}
-        self.log_alpha = torch.full((1,), float(log_alpha), requires_grad=True)
+        self.q1t = {k: to(v) for k, v in (q1_target or q1).items()}
+        self.q2t = {k: to(v) for k, v in (q2_target or q2).items()}
+        self.log_alpha = torch.full((1,), float(log_alpha), dtype=dtype, device=device, requires_grad=True)
+        low, high = low.to(device, dtype), high.to(device, dtype)
         self.popt = torch.optim.Adam([self.pol[k] for k in POLICY_KEYS], lr=lr)
         self.qopt = torch.optim.Adam([self.q1[k] for k in Q_KEYS] + [self.q2[k] for k in Q_KEYS], lr=lr)
         self.aopt = torch.optim.Adam([self.log_alpha], lr=lr)
@@ -91,6 +95,8 @@ class Learner:
         q_loss = (F.mse_loss(q1, y) + F.mse_loss(q2, y)) / 2
         self.qopt.zero_grad()
         q_loss.backward()
+        # the critic gradient of this update: policy_loss.backward() below accumulates into the same .grad tensors
+        self.q_grads = ({k: self.q1[k].grad.clone() for k in Q_KEYS}, {k: self.q2[k].grad.clone() for k in Q_KEYS})
         n1 = math.sqrt(sum(float(self.q1[k].grad.norm(2) ** 2) for k in Q_KEYS))
         n2 = math.sqrt(sum(float(self.q2[k].grad.norm(2) ** 2) for k in Q_KEYS))
         self.qopt.step()

@@ -6,7 +6,8 @@
 //   policy [Pp]: W1[H,O] b1[H] W2[H,H] b2[H] Wm[A,H] Ws[A,H] bm[A] bs[A]      (Wm|Ws adjacent: the two heads are one [2A,H] GEMM)
 //   q      [4][Pq]: W1[H,O+A] b1[H] W2[H,H] b2[H] W3[H] b3[1], order q1, q2, q1_target, q2_target (online nets first: one Adam over 2*Pq)
 // At batch 4096 / hidden 256 the update is launch-latency-bound (SURVEY.md §8 a15), so the value here is that the ~45 launches
-// are issued back-to-back from C++; the GEMMs go through the exact-fp32 SIMT engine (gemm_simt.cuh) with ReLU epilogues.
+// are issued back-to-back from C++.  Forward and input-gradient GEMMs go through run_gemm (gemm_dispatch.cuh): the wgmma 3xTF32 engine
+// under rlx_set_gemm_engine(1) where it covers the shape, the exact-fp32 SIMT engine otherwise; weight gradients always run SIMT.
 #include "common.cuh"
 #include "gemm_simt.cuh"
 #include "gemm_dispatch.cuh"
@@ -185,15 +186,18 @@ __global__ void __launch_bounds__(256) sac_reduce_partials_kernel(float* __restr
 }
 
 // Adam without clipping on a flat buffer (ref: optim.Adam defaults, sac.py:75-77); step counter incremented by thread 0 of block 0 of
-// the preceding sumsq kernel.  norms_out[seg] = sum of squares of segment seg (for logging only).
-__global__ void __launch_bounds__(256) sac_sumsq_step_kernel(const float* __restrict__ g, long long n, long long seg_len, int nseg, float* __restrict__ out,
-                                                             long long* step) {
+// the preceding sumsq kernel.  norms_out[seg] = sum of squares of the first `valid` elements of segment seg (for logging only).  The
+// elements [valid, seg_len) of each segment are the pad of a per-net stride that no gradient kernel writes: they are set to zero here,
+// so that whatever the caller's buffer held there, the norm and the Adam step that follows never see it.
+__global__ void __launch_bounds__(256) sac_sumsq_step_kernel(float* __restrict__ g, long long n, long long seg_len, long long valid, int nseg,
+                                                             float* __restrict__ out, long long* step) {
   __shared__ float sh[34];
   const int seg = blockIdx.x;
   float s = 0.f;
   if (seg < nseg) {
-    const float* p = g + seg * seg_len;
-    for (long long i = threadIdx.x; i < seg_len; i += blockDim.x) s = fmaf(p[i], p[i], s);
+    float* p = g + seg * seg_len;
+    for (long long i = threadIdx.x; i < valid; i += blockDim.x) s = fmaf(p[i], p[i], s);
+    for (long long i = valid + threadIdx.x; i < seg_len; i += blockDim.x) p[i] = 0.f;
   }
   s = block_sum(s, sh);
   if (threadIdx.x == 0) {
@@ -397,7 +401,7 @@ extern "C" int rlx_sac_update_f32(const rlx_sac_update_args* a, void* stream) {
   if ((rc = layer_bwd_input(w.dz2, H, B * H, a->q + L.qW2, H, L.Pq, w.qh1, H, B * H, w.dz1, H, B * H, (int)B, H, H, 2, st))) return rc;
   if ((rc = layer_bwd_weight(w.dz1, H, B * H, w.xa, OA, 0, (int)B, H, OA, 2, w.part, w.rs, gq + L.qW1, gq + L.qb1, L.Pq, st))) return rc;
   // -- grad norms (logging) + Adam over q1 U q2
-  RLX_LAUNCH_C(KC_CLIP_ADAM, 0, 0, sac_sumsq_step_kernel, 2, 256, 0, st, gq, 2 * L.Pq, L.Pq, 2, w.ss + 1, (long long*)a->steps + 1);
+  RLX_LAUNCH_C(KC_CLIP_ADAM, 0, 0, sac_sumsq_step_kernel, 2, 256, 0, st, gq, 2 * L.Pq, L.Pq, L.qb3 + 1, 2, w.ss + 1, (long long*)a->steps + 1);
   RLX_LAUNCH_C(KC_CLIP_ADAM, 0, 28.0 * 2 * L.Pq, sac_adam_kernel, (unsigned)ceil_div(2 * L.Pq, 256), 256, 0, st, a->q, gq, a->m_q, a->v_q, 2 * L.Pq, a->lr,
                (const long long*)a->steps + 1, a->adam_beta1, a->adam_beta2, a->adam_eps);
   // ================================================================ Polyak (sac.py:238-242)
@@ -422,11 +426,11 @@ extern "C" int rlx_sac_update_f32(const rlx_sac_update_args* a, void* stream) {
   if ((rc = layer_bwd_weight(w.pdz2, H, 0, w.ph1, H, 0, (int)B, H, H, 1, w.part, w.rs, gp + L.pW2, gp + L.pb2, 0, st))) return rc;
   if ((rc = layer_bwd_input(w.pdz2, H, 0, a->policy + L.pW2, H, 0, w.ph1, H, 0, w.pdz1, H, 0, (int)B, H, H, 1, st))) return rc;
   if ((rc = layer_bwd_weight(w.pdz1, H, 0, a->states, O, 0, (int)B, H, O, 1, w.part, w.rs, gp + L.pW1, gp + L.pb1, 0, st))) return rc;
-  RLX_LAUNCH_C(KC_CLIP_ADAM, 0, 0, sac_sumsq_step_kernel, 1, 256, 0, st, gp, L.Pp, L.Pp, 1, w.ss, (long long*)a->steps);
+  RLX_LAUNCH_C(KC_CLIP_ADAM, 0, 0, sac_sumsq_step_kernel, 1, 256, 0, st, gp, L.Pp, L.Pp, L.Pp, 1, w.ss, (long long*)a->steps);
   RLX_LAUNCH_C(KC_CLIP_ADAM, 0, 28.0 * L.Pp, sac_adam_kernel, (unsigned)ceil_div(L.Pp, 256), 256, 0, st, a->policy, gp, a->m_policy, a->v_policy, L.Pp, a->lr,
                (const long long*)a->steps, a->adam_beta1, a->adam_beta2, a->adam_eps);
   // -- temperature
-  RLX_LAUNCH_C(KC_CLIP_ADAM, 0, 0, sac_sumsq_step_kernel, 1, 256, 0, st, a->g_log_alpha, 1, 1, 1, w.ss + 3, (long long*)a->steps + 2);
+  RLX_LAUNCH_C(KC_CLIP_ADAM, 0, 0, sac_sumsq_step_kernel, 1, 256, 0, st, a->g_log_alpha, 1, 1, 1, 1, w.ss + 3, (long long*)a->steps + 2);
   RLX_LAUNCH_C(KC_CLIP_ADAM, 0, 0, sac_adam_kernel, 1, 256, 0, st, a->log_alpha, a->g_log_alpha, a->m_log_alpha, a->v_log_alpha, 1, a->lr,
                (const long long*)a->steps + 2, a->adam_beta1, a->adam_beta2, a->adam_eps);
   RLX_LAUNCH(sac_finish_metrics_kernel, 1, 32, 0, st, w.ss, w.ss + 1, a->metrics);
