@@ -8,20 +8,21 @@
 // 3xTF32 does not) at one third of the TF32 tensor rate.
 //
 // Structure (one persistent CTA per SM, 384 threads = 3 warpgroups, static tile schedule, 128 x 128 output tiles):
-//   warpgroup 0   thread 0 issues cp.async.bulk.tensor 2-D tiles (SWIZZLE_128B) of raw fp32 A and B into a 3-stage ring; all 128 threads
-//                 then write the hi and lo tiles of B, K-major and 128-byte swizzled (the only shared-memory layout wgmma accepts for
-//                 tf32), into a 4-stage operand ring and fence.proxy.async it for the tensor core
-//   warpgroups 1, 2   rows 0-63 / 64-127 of the tile: read their A fragments straight from the raw stage, split them into hi / lo in
+//   warpgroup 0   thread 0 issues cp.async.bulk.tensor 2-D tiles (SWIZZLE_128B) of raw fp32 A and B into a 3-stage ring
+//   warpgroups 1, 2   rows 0-63 / 64-127 of the tile: while the MMAs of a k-block's first half run, every consumer thread writes its
+//                 share (1/256) of the NEXT k-block's hi and lo B tiles, K-major and 128-byte swizzled (the only shared-memory layout
+//                 wgmma accepts for tf32), into a 4-stage operand ring; each warp fences its writes for the tensor core and arrives on
+//                 the slot's full barrier on its own.  They read their A fragments straight from the raw stage, split them into hi / lo in
 //                 registers, and issue wgmma.mma_async m64n128k8 tf32 with A from registers (3 per k-slice of 8), keeping one half k-block
 //                 of MMAs in flight while the next half's fragments are loaded; then the epilogue straight from the accumulator registers: bias+tanh / tanh' /
 //                 relu / plain, stores to C (or C^T)
-// A raw slot is refilled once the converter has used its B and all 8 consumer warps hold its A in registers; an operand slot once the
-// wgmmas that read it have retired.
+// A raw slot is refilled once all 8 consumer warps hold its A in registers (each converted its share of the slot's B one k-block
+// before); an operand slot once the wgmmas that read it have retired.
 // Pre-split instances (SPLIT_B: B is a weight matrix whose tf32 hi / lo copies tf32_split made in global memory, K-major): thread 0
-// TMA-loads A, hi B and lo B into one stage [A | hi B | lo B] of a 4-stage ring, which is exactly the layout the converter would have
-// written; warpgroup 0 does no conversion, and a stage is refilled once the wgmmas that read it have retired.
+// TMA-loads A, hi B and lo B into one stage [A | hi B | lo B] of a 4-stage ring, which is exactly the layout the conversion would have
+// written; nothing is converted, and a stage is refilled once the wgmmas that read it have retired.
 // Operand layouts in global memory: K-major (row = m or n, 32 consecutive k = one 128-byte swizzle row) or MN-major (row = k, 32
-// consecutive m/n per 128-byte row; used by the weight-gradient GEMMs whose reduction runs over the minibatch rows).  The converter
+// consecutive m/n per 128-byte row; used by the weight-gradient GEMMs whose reduction runs over the minibatch rows).  The conversion
 // transposes MN-major B tiles to K-major; the consumers' fragment reads transpose MN-major A.  Out-of-bounds parts of a box are
 // zero-filled by TMA, so M / N / K tails need no special code in the main loop.
 #include "gemm_dispatch.cuh"
@@ -37,7 +38,8 @@ struct Cfg {
   static constexpr int B_BYTES = BN * BK * 4;                   // 16 KB
   static constexpr int RAW_BYTES = A_BYTES + B_BYTES;           // raw stage: [A | B] as TMA wrote them
   static constexpr int OP_BYTES = 2 * B_BYTES;                  // operand stage: [hi B | lo B], K-major swizzled
-  // the consumers hold up to two operand slots (the k-block being issued and the one retiring), so 4 stages let the converter run two ahead
+  // in use at once: the slot retiring, the slot being issued and the next k-block's slot being written; the 4th stage lets a warp write
+  // k-block g + 1 once every warp has retired g - 3, so the two consumer warpgroups may drift apart by a k-block without waiting
   static constexpr int RAW_STAGES = 3, OP_STAGES = 4;
   static constexpr int SMEM_BYTES = RAW_STAGES * RAW_BYTES + OP_STAGES * OP_BYTES + 1024 /*barriers*/ + 1024 /*alignment slack*/;
   // pre-split B: stage [A | hi B | lo B]; the consumers hold up to two stages, so 4 stages let the TMA run two ahead
@@ -50,48 +52,54 @@ struct Cfg {
 static_assert(Cfg::SMEM_BYTES <= 227 * 1024 && Cfg::SPLIT_SMEM_BYTES <= 227 * 1024, "shared memory of one H100 block");
 static_assert(Cfg::PRODUCER_REGS * 128 + Cfg::CONSUMER_REGS * 256 <= 65536, "register file of one SM");
 
-// One B tile (ROWS x BK) from its raw stage to K-major swizzled hi / lo tiles.  In the 128-byte swizzle every 16-byte chunk
-// (4 k-values) c of row r sits at r * 128 + ((c ^ (r & 7)) << 4).  Thread t of the warpgroup handles chunks t, t + 128, ...
-template <bool KMAJ, bool BF16, int ROWS>
-__device__ __forceinline__ void convert_tile(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int t) {
-  constexpr uint32_t HI = 0xFFFFE000u;
+// B tile (BN x BK) from its raw stage to K-major swizzled hi / lo tiles, split over the 256 consumer threads.  In the 128-byte swizzle
+// every 16-byte chunk (4 k-values) c of row r sits at r * 128 + ((c ^ (r & 7)) << 4).  Consumer thread t (0..255) handles chunks
+// t + 256 j, j = 0..3.  K-major: TMA wrote the tile in exactly the target layout, an element-wise pass.  MN-major: BN / 32 boxes of
+// [BK k-rows][32 mn] (4 KB each, swizzled the same way with k as the row); chunk i is row mn = i % BN, k-chunk kc = i / BN, so thread t
+// keeps row t % 128 and takes k-chunks t / 128 + 2 j.  A warp handles 32 consecutive mn of one k-chunk: its reads of one k-row hit 32
+// different banks, its 16-byte writes are conflict-free per quarter warp.  Every swizzle term repeats with j (k & 7 does not depend on
+// j, and kc ^ (mn & 7) flips only bits 1-2 with j), so the thread's offsets are computed once: reads of j at rd[q] + 1024 j, the write of
+// j at wr ^ (32 j).  K-major: rd[0] = wr = 16 t, both advancing by 4096 per j.
+template <bool KMAJ>
+__device__ __forceinline__ void b_conv_offsets(int t, uint32_t (&rd)[4], uint32_t& wr) {
   if (KMAJ) {
-    // TMA wrote the tile in exactly the target layout: an element-wise pass
-#pragma unroll 4
-    for (int i = t; i < ROWS * 8; i += 128) {
-      const uint4 v = reinterpret_cast<const uint4*>(raw)[i];
-      const uint4 h = make_uint4(v.x & HI, v.y & HI, v.z & HI, v.w & HI);
-      reinterpret_cast<uint4*>(hi)[i] = h;
-      if (!BF16)
-        reinterpret_cast<float4*>(lo)[i] = make_float4(__uint_as_float(v.x) - __uint_as_float(h.x), __uint_as_float(v.y) - __uint_as_float(h.y),
-                                                       __uint_as_float(v.z) - __uint_as_float(h.z), __uint_as_float(v.w) - __uint_as_float(h.w));
-    }
+    rd[0] = rd[1] = rd[2] = rd[3] = wr = 16u * t;
   } else {
-    // ROWS / 32 boxes of [BK k-rows][32 mn] (4 KB each, swizzled the same way with k as the row).  A warp handles 32 consecutive mn of
-    // one k-chunk: its reads of one k-row hit 32 different banks, its 16-byte writes are conflict-free per quarter warp.
-#pragma unroll 2
-    for (int i = t; i < ROWS * 8; i += 128) {
-      const int mn = i % ROWS, kc = i / ROWS;
-      const uint8_t* box = raw + (mn >> 5) * (BK * 128);
-      const int c = (mn & 31) >> 2, e = mn & 3;
-      uint32_t v[4];
+    const int mn = t & 127, kh = t >> 7;
+    const int c = (mn & 31) >> 2, e = mn & 3;
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const int k = kc * 4 + q;
-        v[q] = *reinterpret_cast<const uint32_t*>(box + k * 128 + ((c ^ (k & 7)) << 4) + e * 4);
-      }
-      const int off = mn * 128 + ((kc ^ (mn & 7)) << 4);
-      const uint4 h = make_uint4(v[0] & HI, v[1] & HI, v[2] & HI, v[3] & HI);
-      *reinterpret_cast<uint4*>(hi + off) = h;
-      if (!BF16)
-        *reinterpret_cast<float4*>(lo + off) = make_float4(__uint_as_float(v[0]) - __uint_as_float(h.x), __uint_as_float(v[1]) - __uint_as_float(h.y),
-                                                           __uint_as_float(v[2]) - __uint_as_float(h.z), __uint_as_float(v[3]) - __uint_as_float(h.w));
+    for (int q = 0; q < 4; ++q) {
+      const int k = 4 * kh + q;
+      rd[q] = (mn >> 5) * (BK * 128) + k * 128 + ((c ^ (k & 7)) << 4) + e * 4;
     }
+    wr = mn * 128 + ((kh ^ (mn & 7)) << 4);
+  }
+}
+
+template <bool KMAJ, bool BF16>
+__device__ __forceinline__ void convert_b(const uint8_t* raw, uint8_t* hi, uint8_t* lo, const uint32_t (&rd)[4], uint32_t wr) {
+  constexpr uint32_t HI = 0xFFFFE000u;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    uint32_t v[4];
+    if (KMAJ) {
+      const uint4 x = *reinterpret_cast<const uint4*>(raw + rd[0] + 4096 * j);
+      v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w;
+    } else {
+#pragma unroll
+      for (int q = 0; q < 4; ++q) v[q] = *reinterpret_cast<const uint32_t*>(raw + rd[q] + 1024 * j);
+    }
+    const uint32_t off = KMAJ ? wr + 4096 * j : wr ^ (32 * j);
+    const uint4 h = make_uint4(v[0] & HI, v[1] & HI, v[2] & HI, v[3] & HI);
+    *reinterpret_cast<uint4*>(hi + off) = h;
+    if (!BF16)
+      *reinterpret_cast<float4*>(lo + off) = make_float4(__uint_as_float(v[0]) - __uint_as_float(h.x), __uint_as_float(v[1]) - __uint_as_float(h.y),
+                                                         __uint_as_float(v[2]) - __uint_as_float(h.z), __uint_as_float(v[3]) - __uint_as_float(h.w));
   }
 }
 
 // A fragments of one half k-block (k-slices 2 half, 2 half + 1) for one consumer thread, from the raw stage, split into hi / lo (the
-// same split as convert_tile).  The thread holds rows r0 and r0 + 8 (r0 = row within the tile, r0 % 8 = lane / 4) at
+// same split as convert_b).  The thread holds rows r0 and r0 + 8 (r0 = row within the tile, r0 % 8 = lane / 4) at
 // k = lane % 4 + 4 j, j = 4 half + jj: k-slice of the half jj / 2, fragment register 2 (jj & 1) + row (see wgmma_tf32_m64n128k8).
 template <bool KMAJ, bool BF16>
 __device__ __forceinline__ void load_a_frags(const uint8_t* raw, int r0, int lane, int half, uint32_t (&hi)[2][4], uint32_t (&lo)[2][4]) {
@@ -238,13 +246,20 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_b);
     if (SPLIT_B) prefetch_tmap(&tmap_b_lo);
+    // Every consumer warp converts a share of each k-block's B (k-block g + 1 while it issues the MMAs of g) and reads the k-block's A.
+    //   raw_full:  1 = thread 0's arrive.expect_tx (the TMA bytes complete it)
+    //   raw_empty: 8 = one arrival per consumer warp once it holds the k-block's A; its B share was converted one k-block earlier in
+    //              the same warp's program order, so all 8 arrivals mean both halves of the raw stage are read
+    //   op_full:   8 = one arrival per consumer warp after its B share is written and fenced for the async proxy
+    //   op_empty:  8 = one arrival per consumer warp once the wgmmas that read the slot have retired
+    // SPLIT_B uses raw_full / op_empty only (one ring, no conversion).
     for (int s = 0; s < RAW_STAGES; ++s) {
       mbar_init(&raw_full[s], 1);
-      mbar_init(&raw_empty[s], 1 + 8);  // the converter + one arrival per consumer warp
+      mbar_init(&raw_empty[s], 8);
     }
     for (int s = 0; s < OP_STAGES; ++s) {
-      mbar_init(&op_full[s], 1);
-      mbar_init(&op_empty[s], 8);  // one arrival per consumer warp
+      mbar_init(&op_full[s], 8);
+      mbar_init(&op_empty[s], 8);
     }
     fence_barrier_init();
   }
@@ -265,9 +280,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
   };
 
   if (warp < 4) {
-    // ===================================================== TMA (thread 0) + B hi / lo converter (warpgroup 0)
+    // ===================================================== TMA (thread 0 of warpgroup 0)
     setmaxnreg_dec<Cfg::PRODUCER_REGS>();
-    const int t = threadIdx.x;
     // load cursor: the k-blocks of this CTA's tiles in consumption order; a raw slot is refilled once its raw_empty phase completes
     // (SPLIT_B: once its op_empty phase completes).  Returns false past the last k-block.
     uint64_t* ld_empty = SPLIT_B ? op_empty : raw_empty;
@@ -307,40 +321,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
       }
       return false;
     };
-    if constexpr (SPLIT_B) {
-      // nothing to convert: thread 0 streams the k-blocks through the ring, the rest of the warpgroup is done
-      if (t == 0)
-        while (load_next()) {
-        }
-      return;
-    }
-    if (t == 0)
-      for (int i = 0; i < RAW_STAGES; ++i) load_next();
-    int rs = 0, os = 0;
-    uint32_t rph = 0, oph = 0;
-    bool refill = false;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      int zb, zs, m0, n0, kbeg, nkb;
-      tile_coords(tile, zb, zs, m0, n0, kbeg, nkb);
-      for (int kb = 0; kb < nkb; ++kb) {
-        mbar_wait(&raw_full[rs], rph);
-        mbar_wait(&op_empty[os], oph ^ 1);
-        uint8_t* op = ops + os * Cfg::OP_BYTES;
-        convert_tile<B_KMAJ, BF16, BN>(smem + rs * Cfg::RAW_BYTES + Cfg::A_BYTES, op, op + Cfg::B_BYTES, t);
-        fence_proxy_async();  // generic-proxy writes -> visible to the tensor core's async-proxy reads
-        named_bar_sync(1, 128);  // the whole warpgroup is done with raw slot rs and has written operand slot os
-        if (t == 0) {
-          mbar_arrive(&op_full[os]);
-          mbar_arrive(&raw_empty[rs]);
-          // refill the PREVIOUS k-block's raw slot: the consumers have usually taken its A by now, so this rarely waits, and the TMA
-          // still runs RAW_STAGES - 1 k-blocks ahead of the converter
-          if (refill) load_next();
-          refill = true;
-        }
-        if (++rs == RAW_STAGES) { rs = 0; rph ^= 1; }
-        if (++os == OP_STAGES) { os = 0; oph ^= 1; }
+    // thread 0 streams the k-blocks through the ring, the rest of the warpgroup is done
+    if (threadIdx.x == 0)
+      while (load_next()) {
       }
-    }
   } else {
     // ===================================================== wgmma consumers + epilogue (warpgroups 1, 2)
     setmaxnreg_inc<Cfg::CONSUMER_REGS>();
@@ -350,12 +334,34 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
     // A fragments of the two half k-blocks that can be in flight: [half][k-slice of the half][register].  Each half is one commit group
     // with registers of its own: a register operand must keep its value until its wgmma retires.
     uint32_t ah[2][2][4], al[2][2][4];
-    int rs = 0, os = 0;
+    // B conversion (not SPLIT_B): this thread's share of k-block g (of the CTA's k-blocks in consumption order, n_kb in all) goes from
+    // raw slot rs to operand slot os, published per warp
+    uint32_t cv_rd[4], cv_wr;
+    b_conv_offsets<B_KMAJ>(threadIdx.x - 128, cv_rd, cv_wr);
+    auto convert_kb = [&](int rs, uint32_t rph, int os, uint32_t oph) {
+      mbar_wait(&raw_full[rs], rph);
+      mbar_wait(&op_empty[os], oph ^ 1);
+      uint8_t* op = ops + os * Cfg::OP_BYTES;
+      convert_b<B_KMAJ, BF16>(smem + rs * Cfg::RAW_BYTES + Cfg::A_BYTES, op, op + Cfg::B_BYTES, cv_rd, cv_wr);
+      fence_proxy_async();  // this thread's generic-proxy writes -> visible to the tensor core's async-proxy reads
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&op_full[os]);
+    };
+    int n_kb = 0;
+    if (!SPLIT_B) {
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        int zb, zs, m0, n0, kbeg, nkb;
+        tile_coords(tile, zb, zs, m0, n0, kbeg, nkb);
+        n_kb += max(nkb, 0);
+      }
+      if (n_kb > 0) convert_kb(0, 0, 0, 0);
+    }
+    int rs = 0, os = 0, g = 0;
     uint32_t rph = 0, oph = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int zb, zs, m0, n0, kbeg, nkb;
       tile_coords(tile, zb, zs, m0, n0, kbeg, nkb);
-      for (int kb = 0; kb < nkb; ++kb) {
+      for (int kb = 0; kb < nkb; ++kb, ++g) {
         mbar_wait(&raw_full[rs], rph);
         if (!SPLIT_B) mbar_wait(&op_full[os], oph);
         const uint8_t* raw = smem + rs * RAW_BYTES;
@@ -384,6 +390,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
             wgmma_tf32_m64n128k8(acc, ah[h][q], db + ko, accum);    // hi * hi  (bf16-valued operands: the whole product)
           }
           wgmma_commit();
+          if (!SPLIT_B && h == 0 && g + 1 < n_kb) {
+            // the next k-block's B share, while this half's MMAs run
+            const bool rw = rs + 1 == RAW_STAGES, ow = os + 1 == OP_STAGES;
+            convert_kb(rw ? 0 : rs + 1, rph ^ (uint32_t)rw, ow ? 0 : os + 1, oph ^ (uint32_t)ow);
+          }
           // the previous half has retired: its A registers may be rewritten, and after the first half the previous k-block's operand
           // slot is free
           wgmma_wait_1();
@@ -483,7 +494,7 @@ static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 static int tc_gemm_impl(const GemmP& g, bool a_kmaj, bool b_kmaj, int epi, int batch, int kclass, long long a_rows, long long b_rows, bool trans,
                         int m_main, float* extra_row, long long extra_batch_off, long long extra_split_off, cudaStream_t stream) {
   if (g.M <= 0 || g.N <= 0) return RLX_OK;
-  // pre-split B (g.b_hi / g.b_lo, K-major [N, K] per batch entry): the instances that exist take it, the rest read g.B through the converter
+  // pre-split B (g.b_hi / g.b_lo, K-major [N, K] per batch entry): the instances that exist take it, the rest convert g.B in the kernel
   const bool split_b = g.b_hi != nullptr && !g.bf16 && !trans && a_kmaj && (epi == TC_EPI_BIAS_TANH || epi == TC_EPI_DTANH);
   if (split_b) {
     if (!aligned16(g.b_hi) || !aligned16(g.b_lo)) return RLX_ERR_UNSUPPORTED;
@@ -598,7 +609,7 @@ __global__ void __launch_bounds__(256) tf32_split_kernel(const __grid_constant__
     const int dr = s.trans ? c0 + i : r0 + i, dc = s.trans ? r0 + tx : c0 + tx, dcols = s.trans ? s.rows : s.cols;
     if (dr < (s.trans ? s.cols : s.rows) && dc < dcols) {
       const float x = s.trans ? tile[tx][i] : tile[i][tx];
-      const uint32_t h = __float_as_uint(x) & 0xFFFFE000u;  // convert_tile's split
+      const uint32_t h = __float_as_uint(x) & 0xFFFFE000u;  // convert_b's split
       const long long o = zoff + (long long)dr * dcols + dc;
       s.hi[o] = __uint_as_float(h);
       s.lo[o] = x - __uint_as_float(h);

@@ -13,7 +13,7 @@ constexpr int BM = 128;        // two consumer warpgroups, 64 rows each (wgmma M
 constexpr int BN = 128;        // wgmma N
 constexpr int BK = 32;         // fp32 elements per k-block = one 128-byte swizzle row
 constexpr int WG_K = 8;        // tf32: 32 bytes of K per wgmma
-constexpr int NUM_THREADS = 384;  // warpgroup 0: TMA + hi/lo converter; warpgroups 1, 2: wgmma consumers + epilogue
+constexpr int NUM_THREADS = 384;  // warpgroup 0: TMA; warpgroups 1, 2: B hi/lo conversion, wgmma consumers + epilogue
 
 enum TcEpi { TC_EPI_NONE = 0, TC_EPI_BIAS_TANH = 1, TC_EPI_DTANH = 2, TC_EPI_BIAS_RELU = 3, TC_EPI_DRELU = 4, TC_EPI_BIAS = 5 };
 
@@ -63,7 +63,6 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* bar, void* smem, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(smem)),
