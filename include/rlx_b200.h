@@ -487,10 +487,25 @@ int rlx_fastsac_normalize_f32(const float* x, int64_t n, int64_t obs_dim, float*
  * Networks (fixed widths like the reference): policy Linear-ReLU x3 (512, 256, 128) + Linear(act) + tanh (policy.py:33-42);
  * Q network Linear-ReLU x3 (1024, 512, 256) + nr_atoms logits on [state | action] (q_network.py:27-35).
  * Flat parameter layouts, torch [out, in] weights in state_dict order:  (W, b) x 4  -> 8 segments each; q buffers hold q1 | q2, the target
- * buffer q1_target | q2_target.  Dense layers go through the aux GEMM engine (rlx_set_aux_gemm_engine). */
+ * buffer q1_target | q2_target.  Dense layers go through the aux GEMM engine (rlx_set_aux_gemm_engine).
+ *
+ * Observation index sets (the env's policy_observation_indices / critic_observation_indices; ref: policy.py:12,26,30,52,
+ * q_network.py:10,22,24,39): the policy reads s[:, policy_idx] (P = policy_in_dim columns), the Q networks [s[:, critic_idx] | a]
+ * (C = critic_in_dim columns, then the actions).  Layer 1 is stored in the reference's shapes, policy [512, P] and Q [1024, C + act], in
+ * the flat parameters, gradients, Adam moments and param_layout.  policy_idx / critic_idx are DEVICE int32 arrays of distinct indices in
+ * [0, obs_dim); the caller validates them.  NULL = identity with in_dim 0 or obs_dim; a non-NULL array needs 1 <= in_dim <= obs_dim.
+ * The states passed to the entry points stay full rows [n, obs_dim].  The selection is an exact column gather, no zero-padded weight:
+ * the Q input is gathered into the padded [s | a] rows (pitch align4(C + act)), the policy input into its own rows at pitch align4(P)
+ * with layer 1's weight staged at that pitch; the actor's gradient through a critic reads the action block at column C of its layer-1
+ * weight.  A zero / NULL tail is the identity network, launch for launch and with the same workspace size. */
 #define RLX_FASTTD3_POLICY_NSEG 8
 #define RLX_FASTTD3_Q_NSEG 8
-typedef struct rlx_fasttd3_dims { int32_t obs_dim, act_dim, nr_atoms; } rlx_fasttd3_dims;
+typedef struct rlx_fasttd3_dims {
+  int32_t obs_dim, act_dim, nr_atoms;
+  int32_t policy_in_dim, critic_in_dim;  /* P, C; 0 = obs_dim */
+  const int32_t* policy_idx;             /* [P] device array, or NULL = identity */
+  const int32_t* critic_idx;             /* [C] device array, or NULL = identity */
+} rlx_fasttd3_dims;
 int rlx_fasttd3_param_layout(const rlx_fasttd3_dims* d, int64_t* policy_offsets /*[9]*/, int64_t* q_offsets /*[9], one network*/);
 size_t rlx_fasttd3_workspace_bytes(const rlx_fasttd3_dims* d, int64_t n);
 

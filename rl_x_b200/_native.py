@@ -149,7 +149,9 @@ RLX_FASTTD3_POLICY_NSEG, RLX_FASTTD3_Q_NSEG = 8, 8
 
 
 class FastTd3Dims(C.Structure):
-    _fields_ = [(n, C.c_int32) for n in ("obs_dim", "act_dim", "nr_atoms")]
+    """rlx_fasttd3_dims.  The tail (observation index sets) defaults to zeros / NULL: both networks read every observation column."""
+    _fields_ = [(n, C.c_int32) for n in ("obs_dim", "act_dim", "nr_atoms", "policy_in_dim", "critic_in_dim")] + \
+               [("policy_idx", C.c_void_p), ("critic_idx", C.c_void_p)]
 
 
 class FastTd3Hparams(C.Structure):

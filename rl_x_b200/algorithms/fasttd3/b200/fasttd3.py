@@ -9,8 +9,12 @@ Host side: Python/PyTorch for device memory and the TORCH-interface environment;
 
 Parameters are initialised exactly like the reference (the same torch modules built in the same order under torch.manual_seed(seed),
 fasttd3.py:81-85) and live in the library's flat layout; the acting noise, smoothing noise and per-environment exploration scales are
-torch.randn / torch.rand on the device, drawn in the reference's order.  Not built: bf16 autocast.  GPU tests:
-tests/test_gpu_zzzzz_fasttd3.py; the same sources are checked in host emulation (tests/test_fasttd3_emulation.py).
+torch.randn / torch.rand on the device, drawn in the reference's order.  The env's policy_observation_indices /
+critic_observation_indices (policy.py:12,52, q_network.py:10,39) are validated on the host and passed to the library as device int32
+arrays: the policy's first layer is [512, P] and each Q network's [1024, C + act], the reference's shapes; the replay buffer and the
+observation normaliser stay full-width.  Not built: bf16 autocast.  GPU tests: tests/test_gpu_zzzzz_fasttd3.py,
+tests/test_gpu_zzzzzzzzzzzzz_fasttd3_obs_indices.py; the same sources are checked in host emulation (tests/test_fasttd3_emulation.py,
+tests/test_fasttd3_obs_indices.py).
 """
 import ctypes as C
 import logging
@@ -22,7 +26,6 @@ import torch
 
 from rl_x_b200 import _native as nt
 from rl_x_b200.algorithms.fastsac.b200.replay_buffer import ReplayBuffer
-from rl_x_b200.environments.types import require_identity_observation_indices
 
 rlx_logger = logging.getLogger("rl_x")
 POLICY_WIDTHS, Q_WIDTHS = (512, 256, 128), (1024, 512, 256)
@@ -32,9 +35,13 @@ def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
-def reference_init(obs, act, nr_atoms, seed):
+def reference_init(obs, act, nr_atoms, seed, policy_in=None, critic_in=None):
     """FastTD3.__init__'s parameter values (fasttd3.py:81-85, policy.py:33-48, critic.py:17-22): same torch modules, construction order and
-    seed.  Returns the flat policy vector and the flat q1 | q2 vector in the layout of include/rlx_b200.h (torch state_dict order)."""
+    seed.  Returns the flat policy vector and the flat q1 | q2 vector in the layout of include/rlx_b200.h (torch state_dict order).
+    policy_in / critic_in: the lengths of the observation index sets (None = obs), the fan-ins of the first layers (policy.py:30,
+    q_network.py:24)."""
+    policy_in = obs if policy_in is None else policy_in
+    critic_in = obs if critic_in is None else critic_in
     torch.manual_seed(seed)
 
     def mlp(inp, widths, out):
@@ -47,10 +54,10 @@ def reference_init(obs, act, nr_atoms, seed):
     def flat(layers):
         return torch.cat([t.detach().reshape(-1) for lyr in layers for t in (lyr.weight, lyr.bias)])
 
-    pol = mlp(obs, POLICY_WIDTHS, act)
+    pol = mlp(policy_in, POLICY_WIDTHS, act)
     torch.nn.init.normal_(pol[-1].weight, 0.0, 0.01)
     torch.nn.init.constant_(pol[-1].bias, 0.0)
-    qs = [flat(mlp(obs + act, Q_WIDTHS, nr_atoms)) for _ in range(4)]   # q1, q2, then the targets, which consume the generator too
+    qs = [flat(mlp(critic_in + act, Q_WIDTHS, nr_atoms)) for _ in range(4)]   # q1, q2, then the targets, which consume the generator too
     return flat(pol), torch.cat(qs[:2])
 
 
@@ -94,7 +101,12 @@ class FastTD3:
             raise ValueError("The save frequency must be a multiple of the number of environments.")
         if a.get("bf16_mixed_precision_training", False):
             raise NotImplementedError("rl_x_b200 FastTD3 implements the reference's fp32 path; set algorithm.bf16_mixed_precision_training=False.")
-        require_identity_observation_indices(self.train_env, "FastTD3")  # policy.py:12 / q_network.py:10,39
+        # the networks' input columns (policy.py:12,52 / q_network.py:10,39): validated on the host before any device work; None = identity
+        obs = int(self.train_env.single_observation_space.shape[0])
+        self.policy_observation_indices = nt.observation_indices(
+            "policy_observation_indices", getattr(self.train_env, "policy_observation_indices", None), obs)
+        self.critic_observation_indices = nt.observation_indices(
+            "critic_observation_indices", getattr(self.train_env, "critic_observation_indices", None), obs)
         if a.device != "gpu" or not torch.cuda.is_available():
             raise RuntimeError("rl_x_b200 FastTD3 needs a CUDA device (algorithm.device=gpu); there is no CPU fallback.")
         self.device = torch.device("cuda", torch.cuda.current_device())
@@ -106,14 +118,23 @@ class FastTD3:
             raise ValueError("algorithm.gemm_engine must be auto, simt or tcgen05")
         if engine != "auto":
             self.lib.rlx_set_aux_gemm_engine(1 if engine == "tcgen05" else 0)
-        obs, act = int(self.train_env.single_observation_space.shape[0]), int(np.prod(self.train_env.single_action_space.shape))
+        act = int(np.prod(self.train_env.single_action_space.shape))
         self.dims = nt.FastTd3Dims(obs, act, int(a.nr_atoms))
+        # device copies of the index sets, kept alive for as long as self.dims points at them
+        self._idx = {}
+        for k, ind in (("policy", self.policy_observation_indices), ("critic", self.critic_observation_indices)):
+            if ind is not None:
+                self._idx[k] = torch.as_tensor(ind, dtype=torch.int32).to(self.device).contiguous()
+                setattr(self.dims, f"{k}_in_dim", int(ind.size))
+                setattr(self.dims, f"{k}_idx", self._idx[k].data_ptr())
+        self.policy_in = obs if self.policy_observation_indices is None else int(self.policy_observation_indices.size)
+        self.critic_in = obs if self.critic_observation_indices is None else int(self.critic_observation_indices.size)
         poff, qoff = (C.c_int64 * (nt.RLX_FASTTD3_POLICY_NSEG + 1))(), (C.c_int64 * (nt.RLX_FASTTD3_Q_NSEG + 1))()
         nt.check(self.lib.rlx_fasttd3_param_layout(C.byref(self.dims), poff, qoff), "rlx_fasttd3_param_layout")
         self.policy_offsets, self.q_offsets = list(poff), list(qoff)
 
         self.rng = np.random.default_rng(self.seed)
-        policy, q = reference_init(obs, act, int(a.nr_atoms), self.seed)   # torch.manual_seed(self.seed) inside, as fasttd3.py:81
+        policy, q = reference_init(obs, act, int(a.nr_atoms), self.seed, self.policy_in, self.critic_in)   # torch.manual_seed(self.seed) inside, as fasttd3.py:81
         assert policy.numel() == self.policy_offsets[-1] and q.numel() == 2 * self.q_offsets[-1]
         dev = self.device
         self.policy_params, self.q_params = policy.to(dev).contiguous(), q.to(dev).contiguous()
@@ -341,8 +362,8 @@ class FastTD3:
     # The reference's file layout and state_dict key names (fasttd3.py:449-482), so that models move between the two implementations.
     def _named(self, flat, net):
         """flat parameter-like vector -> {state_dict key: tensor} for "policy" or one Q network."""
-        obs, act, atoms = self.dims.obs_dim, self.dims.act_dim, self.dims.nr_atoms
-        widths, inp, out, prefix = (POLICY_WIDTHS, obs, act, "policy") if net == "policy" else (Q_WIDTHS, obs + act, atoms, "critic")
+        act, atoms = self.dims.act_dim, self.dims.nr_atoms
+        widths, inp, out, prefix = (POLICY_WIDTHS, self.policy_in, act, "policy") if net == "policy" else (Q_WIDTHS, self.critic_in + act, atoms, "critic")
         shapes, last = [], inp
         for k, w in enumerate(tuple(widths) + (out,)):
             shapes += [(f"{prefix}.{2 * k}.weight", (w, last)), (f"{prefix}.{2 * k}.bias", (w,))]

@@ -16,14 +16,16 @@ constexpr int kWgradRows = 1024;   // rows per split of the weight-gradient GEMM
 
 #define C51_TRY(expr) do { int _rc = (expr); if (_rc) return _rc; } while (0)
 
-// XA[r, :O+Ad] = [X | A] with row pitch ld (columns >= O + Ad are not written).  thread = element
-static __global__ void concat_kernel(const float* __restrict__ X, const float* __restrict__ A, long long n, int O, int Ad, int ld, float* __restrict__ XA) {
+// XA[r, :O+Ad] = [X | A] with row pitch ld (columns >= O + Ad are not written).  idx (nullable): the O observation columns are the
+// gathered X[r, idx[k]] of rows at pitch ldX (an observation index set); NULL: X[r, k] at pitch O.  thread = element
+static __global__ void concat_kernel(const float* __restrict__ X, const float* __restrict__ A, long long n, int O, int Ad, int ld, float* __restrict__ XA,
+                                     const int32_t* __restrict__ idx = nullptr, int ldX = 0) {
   const long long id = gtid();
   const int W = O + Ad;
   if (id >= n * W) return;
   const long long r = id / W;
   const int k = (int)(id % W);
-  XA[r * ld + k] = k < O ? X[r * O + k] : A[r * Ad + (k - O)];
+  XA[r * ld + k] = k >= O ? A[r * Ad + (k - O)] : idx ? X[r * ldX + idx[k]] : X[r * O + k];
 }
 // dAct[r, a] = dXA0[r, O + a] + dXA1[r, O + a]: the action columns of the two critics' input gradients (row pitch ld).  thread = element
 static __global__ void action_grad_kernel(const float* __restrict__ dXA0, const float* __restrict__ dXA1, long long n, int O, int A, int ld,

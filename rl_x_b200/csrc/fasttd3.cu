@@ -28,21 +28,33 @@ static void mlp_layout(long long* off, int in, const int* widths, int out) {
   }
   off[s] = o;
 }
+// Observation widths of layer 1 (include/rlx_b200.h): P of the policy, C of the Q networks; obs_dim where the index set is the identity.
+// Elsewhere obs_dim is only the row width of the replay states the sets index into.
+static int pol_in(const rlx_fasttd3_dims& d) { return d.policy_idx ? d.policy_in_dim : d.obs_dim; }
+static int crit_in(const rlx_fasttd3_dims& d) { return d.critic_idx ? d.critic_in_dim : d.obs_dim; }
 static Layout make_layout(const rlx_fasttd3_dims& d) {
   Layout l;
-  mlp_layout(l.p, d.obs_dim, kPW, d.act_dim);
-  mlp_layout(l.q, d.obs_dim + d.act_dim, kQW, d.nr_atoms);
+  mlp_layout(l.p, pol_in(d), kPW, d.act_dim);
+  mlp_layout(l.q, crit_in(d) + d.act_dim, kQW, d.nr_atoms);
   return l;
 }
-static bool dims_ok(const rlx_fasttd3_dims& d) { return d.obs_dim > 0 && d.act_dim > 0 && d.act_dim <= 64 && d.nr_atoms >= 2 && d.nr_atoms <= 1024; }
+static bool set_ok(int32_t in, const int32_t* idx, int32_t obs) { return idx ? in >= 1 && in <= obs : in == 0 || in == obs; }
+static bool dims_ok(const rlx_fasttd3_dims& d) {
+  return d.obs_dim > 0 && d.act_dim > 0 && d.act_dim <= 64 && d.nr_atoms >= 2 && d.nr_atoms <= 1024 && set_ok(d.policy_in_dim, d.policy_idx, d.obs_dim) &&
+         set_ok(d.critic_in_dim, d.critic_idx, d.obs_dim);
+}
 // row pitch of the [s | a] buffers and of the staged layer-1 Q weights: a multiple of 4 floats (16 B), which a TMA descriptor needs
-static int xa_pitch(const rlx_fasttd3_dims& d) { return (int)align_up((size_t)(d.obs_dim + d.act_dim), 4); }
+static int xa_pitch(const rlx_fasttd3_dims& d) { return (int)align_up((size_t)(crit_in(d) + d.act_dim), 4); }
+// the same for the gathered policy input s[:, policy_idx] and its staged layer-1 weight (only with a policy index set)
+static int sp_pitch(const rlx_fasttd3_dims& d) { return (int)align_up((size_t)pol_in(d), 4); }
 
 struct Ws {
-  size_t pH[3], qH[2][3], XA, Act, Logits[2], Proj[2], dLogits, dA, dB, dXa[2], dAct, RowA, RowB, Zero, Small, W1[2], QP[2], Part, Col, total;
+  size_t pH[3], qH[2][3], XA, Act, Logits[2], Proj[2], dLogits, dA, dB, dXa[2], dAct, RowA, RowB, Zero, Small, W1[2], QP[2], Part, Col, SP, W1p, total;
 };
 static Ws plan(const rlx_fasttd3_dims& d, long long n_) {
-  const size_t n = (size_t)n_, O = d.obs_dim, A = d.act_dim, K = d.nr_atoms, P = (size_t)xa_pitch(d);
+  const size_t n = (size_t)n_, A = d.act_dim, K = d.nr_atoms, P = (size_t)xa_pitch(d);
+  // layer-1 weight-gradient partials of the policy: at the gathered input's pitch with a set, at obs_dim (states read in place) without
+  const size_t pol_ld = d.policy_idx ? (size_t)sp_pitch(d) : (size_t)d.obs_dim, sp = d.policy_idx ? (size_t)sp_pitch(d) : 0;
   Ws w;
   size_t o = 0;
   auto take = [&](size_t& f, size_t cnt) { f = o; o += align_up(cnt, 64); };
@@ -58,10 +70,11 @@ static Ws plan(const rlx_fasttd3_dims& d, long long n_) {
   take(w.QP[0], nq); take(w.QP[1], nq);   // aligned_params: a critic's parameter block when its base is not 16-byte aligned
   const size_t splits = (size_t)ceil_div((long long)n, kWgradRows);
   size_t biggest = std::max<size_t>((size_t)kQW[0] * P, (size_t)kQW[1] * kQW[0]);
-  biggest = std::max<size_t>(biggest, std::max<size_t>((size_t)kPW[0] * O, (size_t)K * kQW[2]));
+  biggest = std::max<size_t>(biggest, std::max<size_t>((size_t)kPW[0] * pol_ld, (size_t)K * kQW[2]));
   take(w.Part, splits * biggest);
   const size_t chunks = (size_t)ceil_div((long long)n, kColChunk);
   take(w.Col, chunks * std::max<size_t>(1024, std::max<size_t>(K, 8)));
+  take(w.SP, n * sp); take(w.W1p, (size_t)kPW[0] * sp);   // empty without a policy index set: the workspace is the identity network's
   w.total = o * sizeof(float);
   return w;
 }
@@ -70,6 +83,16 @@ static Ws plan(const rlx_fasttd3_dims& d, long long n_) {
 static __global__ void fill_kernel(float* __restrict__ x, long long n, float v) {
   const long long i = gtid();
   if (i < n) x[i] = v;
+}
+// dst[r, j] = src[r * ld_src + idx[j]] for j < cols, dst at row pitch ld (the policy's input s[:, policy_idx]; pad columns not written).
+// thread = element
+static __global__ void gather_cols_kernel(const float* __restrict__ src, long long rows, int ld_src, const int32_t* __restrict__ idx, int cols, int ld,
+                                          float* __restrict__ dst) {
+  const long long id = gtid();
+  if (id >= rows * cols) return;
+  const long long r = id / cols;
+  const int j = (int)(id % cols);
+  dst[r * ld + j] = src[r * ld_src + idx[j]];
 }
 // dst[r, :cols] = src[r, :cols] with row pitch ld (the padded copy of a layer-1 weight).  thread = element
 static __global__ void pitch_copy_kernel(const float* __restrict__ src, long long rows, int cols, int ld, float* __restrict__ dst) {
@@ -174,15 +197,35 @@ struct Hs { float* h[3]; };
 static Hs hs_p(float* ws, const Ws& w) { return {{ws + w.pH[0], ws + w.pH[1], ws + w.pH[2]}}; }
 static Hs hs_q(float* ws, const Ws& w, int q) { return {{ws + w.qH[q][0], ws + w.qH[q][1], ws + w.qH[q][2]}}; }
 
+// Policy on the states X [n, obs_dim].  Without a policy index set layer 1 reads X and its weight in place.  With one, X[:, policy_idx] is
+// gathered into SP and the [512, P] weight staged into W1p, both at the padded pitch sp_pitch.  *Xin / *ldin: layer 1's input as read (for
+// mlp_bwd's weight gradient; SP stays intact until the next policy forward).
 static int policy_fwd(const rlx_fasttd3_dims& d, const Layout& l, const Ws& w, float* ws, const float* P, const float* X, long long n, float* action,
-                      cudaStream_t st) {
+                      cudaStream_t st, const float** Xin = nullptr, int* ldin = nullptr) {
   const Hs h = hs_p(ws, w);
-  return mlp_fwd(P, l.p, kPW, X, d.obs_dim, d.obs_dim, P + l.p[0], d.obs_dim, h.h, d.act_dim, true, action, n, st);
+  const int in = pol_in(d);
+  const float *x = X, *W1 = P + l.p[0];
+  int ld = d.obs_dim;
+  if (d.policy_idx) {
+    ld = sp_pitch(d);
+    RLX_FLAT_LAUNCH(gather_cols_kernel, n * in, st, X, n, d.obs_dim, d.policy_idx, in, ld, ws + w.SP);
+    RLX_FLAT_LAUNCH(pitch_copy_kernel, (long long)kPW[0] * in, st, P + l.p[0], (long long)kPW[0], in, ld, ws + w.W1p);
+    x = ws + w.SP;
+    W1 = ws + w.W1p;
+  }
+  if (Xin) { *Xin = x; *ldin = ld; }
+  return mlp_fwd(P, l.p, kPW, x, ld, in, W1, ld, h.h, d.act_dim, true, action, n, st);
+}
+// [s[:, critic_idx] | a] into the padded rows XA (s at row pitch obs_dim; the identity set copies s whole)
+static int critic_input(const rlx_fasttd3_dims& d, const float* S, const float* Act, long long n, float* XA, cudaStream_t st) {
+  const int C = crit_in(d), A = d.act_dim;
+  RLX_FLAT_LAUNCH(concat_kernel, n * (C + A), st, S, Act, n, C, A, xa_pitch(d), XA, d.critic_idx, d.obs_dim);
+  return RLX_OK;
 }
 // Q network on the padded [s | a] rows: stages the layer-1 weight at the padded pitch into slot `slot`, then the forward
 static int q_fwd(const rlx_fasttd3_dims& d, const Layout& l, const Ws& w, float* ws, const float* Q, int slot, const float* XA, long long n, const Hs& h,
                  float* logits, cudaStream_t st) {
-  const int in = d.obs_dim + d.act_dim, ldx = xa_pitch(d);
+  const int in = crit_in(d) + d.act_dim, ldx = xa_pitch(d);
   RLX_FLAT_LAUNCH(pitch_copy_kernel, (long long)kQW[0] * in, st, Q + l.q[0], (long long)kQW[0], in, ldx, ws + w.W1[slot]);
   return mlp_fwd(Q, l.q, kQW, XA, ldx, in, ws + w.W1[slot], ldx, h.h, d.nr_atoms, false, logits, n, st);
 }
@@ -226,7 +269,7 @@ extern "C" int rlx_fasttd3_critic_update_f32(const rlx_fasttd3_update_args* a, v
   cudaStream_t st = (cudaStream_t)stream;
   const Layout l = make_layout(d);
   const long long n = a->n, nq = l.q[RLX_FASTTD3_Q_NSEG];
-  const int O = d.obs_dim, A = d.act_dim, K = d.nr_atoms, ldx = xa_pitch(d);
+  const int IN = crit_in(d) + d.act_dim, A = d.act_dim, K = d.nr_atoms, ldx = xa_pitch(d);
   float* ws = (float*)a->workspace;
   const rlx_fasttd3_hparams& hp = a->hp;
   float *XA = ws + w.XA, *Act = ws + w.Act, *RowA = ws + w.RowA, *RowB = ws + w.RowB, *Small = ws + w.Small, *Zero = ws + w.Zero;
@@ -234,7 +277,7 @@ extern "C" int rlx_fasttd3_critic_update_f32(const rlx_fasttd3_update_args* a, v
   // ---- target (no gradients): smoothed a' from the online policy, both target networks on (s', a'), projection (fasttd3.py:142-197)
   TD_TRY(policy_fwd(d, l, w, ws, a->policy_params, a->next_states, n, Act, st));
   RLX_FLAT_LAUNCH(smooth_target_action_kernel, n * A, st, Act, a->smoothing_noise, n * A, hp.smoothing_epsilon, hp.smoothing_clip_value);
-  RLX_FLAT_LAUNCH(concat_kernel, n * (O + A), st, a->next_states, Act, n, O, A, ldx, XA);
+  TD_TRY(critic_input(d, a->next_states, Act, n, XA, st));
   for (int q = 0; q < 2; ++q) {
     const float* QT;
     TD_TRY(aligned_params(a->q_target_params + q * nq, nq, ws + w.QP[q], &QT, st));
@@ -248,7 +291,7 @@ extern "C" int rlx_fasttd3_critic_update_f32(const rlx_fasttd3_update_args* a, v
   const long long nchunk = ceil_div(n, kColChunk);
   RLX_FLAT_LAUNCH(minmax_partial_kernel, nchunk, st, RowA, n, RowB);
   // ---- current critics on (s, a): cross-entropy and its gradient (fasttd3.py:199-212)
-  RLX_FLAT_LAUNCH(concat_kernel, n * (O + A), st, a->states, a->actions, n, O, A, ldx, XA);
+  TD_TRY(critic_input(d, a->states, a->actions, n, XA, st));
   const float inv_n = 1.f / (float)n;
   for (int q = 0; q < 2; ++q) {
     const Hs& h = q == 0 ? q0 : q1;
@@ -256,7 +299,7 @@ extern "C" int rlx_fasttd3_critic_update_f32(const rlx_fasttd3_update_args* a, v
     TD_TRY(aligned_params(a->q_params + q * nq, nq, ws + w.QP[q], &Q, st));
     TD_TRY(q_fwd(d, l, w, ws, Q, q, XA, n, h, ws + w.Logits[q], st));
     RLX_FLAT_LAUNCH(ce_rows_kernel, n, st, ws + w.Logits[q], ws + w.Proj[q], n, K, inv_n, RowA + (1 + q) * n, ws + w.dLogits);
-    TD_TRY(mlp_bwd(Q, a->q_grads + q * nq, l.q, kQW, XA, ldx, O + A, h.h, K, ws + w.dLogits, n, ws + w.dA, ws + w.dB, ws + w.Part, ws + w.Col, st));
+    TD_TRY(mlp_bwd(Q, a->q_grads + q * nq, l.q, kQW, XA, ldx, IN, h.h, K, ws + w.dLogits, n, ws + w.dA, ws + w.dB, ws + w.Part, ws + w.Col, st));
   }
   TD_TRY(colsum(RowA + n, 1, n, 1, ws + w.Col, 1.f, 0.f, Small + 0, st));
   TD_TRY(colsum(RowA + 2 * n, 1, n, 1, ws + w.Col, 1.f, 0.f, Small + 1, st));
@@ -276,7 +319,7 @@ extern "C" int rlx_fasttd3_policy_update_f32(const rlx_fasttd3_update_args* a, v
   cudaStream_t st = (cudaStream_t)stream;
   const Layout l = make_layout(d);
   const long long n = a->n, nq = l.q[RLX_FASTTD3_Q_NSEG];
-  const int O = d.obs_dim, A = d.act_dim, K = d.nr_atoms, ldx = xa_pitch(d);
+  const int C = crit_in(d), A = d.act_dim, K = d.nr_atoms;
   float* ws = (float*)a->workspace;
   const rlx_fasttd3_hparams& hp = a->hp;
   float *XA = ws + w.XA, *Act = ws + w.Act, *RowA = ws + w.RowA, *Small = ws + w.Small, *dAct = ws + w.dAct;
@@ -284,8 +327,10 @@ extern "C" int rlx_fasttd3_policy_update_f32(const rlx_fasttd3_update_args* a, v
   const float inv_n = 1.f / (float)n;
   const int clipped = hp.clipped_double_q != 0.f ? 1 : 0;
   // a = pi(s); q = min / mean of E[q1], E[q2] on (s, a); L = -mean(q)   (fasttd3.py:106-120)
-  TD_TRY(policy_fwd(d, l, w, ws, a->policy_params, a->states, n, Act, st));
-  RLX_FLAT_LAUNCH(concat_kernel, n * (O + A), st, a->states, Act, n, O, A, ldx, XA);
+  const float* Xp;
+  int ldp;
+  TD_TRY(policy_fwd(d, l, w, ws, a->policy_params, a->states, n, Act, st, &Xp, &ldp));
+  TD_TRY(critic_input(d, a->states, Act, n, XA, st));
   const float* Qp[2];
   for (int q = 0; q < 2; ++q) {
     TD_TRY(aligned_params(a->q_params + q * nq, nq, ws + w.QP[q], &Qp[q], st));
@@ -304,12 +349,12 @@ extern "C" int rlx_fasttd3_policy_update_f32(const rlx_fasttd3_update_args* a, v
       TD_TRY(lin_bwd_input<EPI_DRELU>(dA, kQW[k], Q + l.q[2 * k], kQW[k - 1], kQW[k], dB, kQW[k - 1], n, st, h.h[k - 1]));
       std::swap(dA, dB);
     }
-    // dAct_q[r, j] = sum_o dA[r, o] W1[o, O + j]: the action block of the first layer's weight, read in place
-    TD_TRY(lin_bwd_input(dA, kQW[0], Q + l.q[0] + O, A, kQW[0], ws + w.dXa[q], A, n, st, nullptr, O + A));
+    // dAct_q[r, j] = sum_o dA[r, o] W1[o, C + j]: the action block of the first layer's weight [1024, C + act], read in place
+    TD_TRY(lin_bwd_input(dA, kQW[0], Q + l.q[0] + C, A, kQW[0], ws + w.dXa[q], A, n, st, nullptr, C + A));
   }
   RLX_FLAT_LAUNCH(action_grad_kernel, n * A, st, ws + w.dXa[0], ws + w.dXa[1], n, 0, A, A, dAct);
   RLX_FLAT_LAUNCH(tanh_bwd_kernel, n * A, st, dAct, Act, n * A, ws + w.dXa[0]);   // dXa[0] is free again: the gradient wrt the pre-tanh head
-  TD_TRY(mlp_bwd(a->policy_params, a->policy_grads, l.p, kPW, a->states, O, O, ph.h, A, ws + w.dXa[0], n, ws + w.dA, ws + w.dB, ws + w.Part, ws + w.Col,
+  TD_TRY(mlp_bwd(a->policy_params, a->policy_grads, l.p, kPW, Xp, ldp, pol_in(d), ph.h, A, ws + w.dXa[0], n, ws + w.dA, ws + w.dB, ws + w.Part, ws + w.Col,
                  st));
   // metrics: policy_loss; then AdamW (its pre-clip gradient norm is metrics[1])
   RLX_FLAT_LAUNCH(combine_values_kernel, n, st, RowA + n, RowA + 2 * n, n, clipped, RowA + 3 * n);
