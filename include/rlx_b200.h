@@ -328,6 +328,20 @@ int rlx_debug_ppo_head_gemm_f32(int64_t m, int32_t hidden, int32_t act_dim, cons
                                 const float* b3c, const float* logstd, const float* actions, const float* logp_old, const float* adv,
                                 const float* ret, const float* adv_stats, float inv_mg, float clip_range, float critic_coef,
                                 int32_t ratio_delta_metric, float* dZ2, float* dhead, float* headpart, float* scratch, void* stream);
+/* The same, with ratio_abs: null, or [m] out = |ratio - 1| per row (what the ESPO median selects from). */
+int rlx_debug_ppo_head_gemm_ratio_f32(int64_t m, int32_t hidden, int32_t act_dim, const float* H2, const float* W3p, const float* W3c,
+                                      const float* b3p, const float* b3c, const float* logstd, const float* actions, const float* logp_old,
+                                      const float* adv, const float* ret, const float* adv_stats, float inv_mg, float clip_range, float critic_coef,
+                                      int32_t ratio_delta_metric, float* dZ2, float* dhead, float* headpart, float* ratio_abs, float* scratch,
+                                      void* stream);
+/* The loss-head kernels the last rlx_ppo_minibatch_fwdbwd_f32 call (or minibatch of an epoch call) launched, into out[6]:
+ *   out[0] train-head kernel: 0 ppo_head_train_kernel, 1 ppo_head_train2_kernel, 2 ppo_head_train3_kernel, 3 ppo_head_train4_kernel,
+ *          4 the GEMM head (csrc/ppo_head_gemm.cu);
+ *   out[1], out[2] its template arguments: NCH or H, then ACT_MAX or NT (0 where the kernel has none);
+ *   out[3] 1 for the BF16 instance;
+ *   out[4] weight-gradient kernel: 0 ppo_head_wgrad_kernel, 1 ppo_head_wgrad3_kernel, 2 the wgmma GEMM;  out[5] its ACT_MAX (0 for the GEMM).
+ * Every entry is -1 when the call launched no head (m == 0, or it failed before the head).  Host-side record of this process. */
+int rlx_debug_ppo_head_path(int32_t* out);
 
 /* ------------------------------------------------------------------------------------------ PPO + LSTM path -- */
 /* SURVEY.md §8 a18: rl_x/algorithms/ppo_lstm/flax (policy.py:36-146, critic.py:18-30, ppo_lstm.py:107-231), including the two policy

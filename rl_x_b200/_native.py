@@ -191,6 +191,8 @@ _SIGNATURES = {
     "rlx_set_gae_tma": (C.c_int, [C.c_int]),
     "rlx_set_autocast_bf16": (C.c_int, [C.c_int]),
     "rlx_debug_ppo_head_gemm_f32": (C.c_int, [C.c_int64, C.c_int32, C.c_int32] + [C.c_void_p] * 11 + [C.c_float] * 3 + [C.c_int32] + [C.c_void_p] * 5),
+    "rlx_debug_ppo_head_gemm_ratio_f32": (C.c_int, [C.c_int64, C.c_int32, C.c_int32] + [C.c_void_p] * 11 + [C.c_float] * 3 + [C.c_int32] + [C.c_void_p] * 6),
+    "rlx_debug_ppo_head_path": (C.c_int, [C.c_void_p]),
     "rlx_get_gemm_engine": (C.c_int, []),
     "rlx_pcg64_seed": (C.c_int, [C.c_uint64, C.POINTER(Pcg64)]),
     "rlx_pcg64_next64": (C.c_uint64, [C.POINTER(Pcg64)]),

@@ -383,6 +383,14 @@ static int launch_grad_reduce(const GradReduceP& r, cudaStream_t st) {
 // the head kernels with the act <= 31 specialisations (and their dW3 kernels) cover the shape
 static bool fast_head_ok(const PpoLayout& L) { return (L.act <= 31) && (L.H % 2 == 0) && (L.H <= 1024); }
 
+// The loss-head kernels the last minibatch call launched (rlx_debug_ppo_head_path): train-head kernel, its two template arguments and
+// BF16 flag, then the weight-gradient kernel and its ACT_MAX.  -1 = not launched.  Set where each instance is launched.
+static int g_head_path[6] = {-1, -1, -1, -1, -1, -1};
+static void record_train_head(int kernel, int t0, int t1, int bf16) {
+  g_head_path[0] = kernel; g_head_path[1] = t0; g_head_path[2] = t1; g_head_path[3] = bf16 ? 1 : 0;
+}
+static void record_head_wgrad(int kernel, int act_max) { g_head_path[4] = kernel; g_head_path[5] = act_max; }
+
 // loss head: loss + dZ2 + dhead + block partials (incl. db2 = column sums of dZ2).  Returns the number of partial blocks written, < 0 on error.
 static int launch_train_head(const rlx_ppo_minibatch_args* a, const PpoLayout& L, const TrainPlan& P, const float* params, int bf16, cudaStream_t st) {
   const long long m = a->m;
@@ -412,13 +420,16 @@ static int launch_train_head(const rlx_ppo_minibatch_args* a, const PpoLayout& L
   if (gemm_head) {
     HeadGemmArgs ha{m, H, A, dh_ld, H2, a->params + L.off[W3P], a->params + L.off[W3C], a->params + L.off[B3P], a->params + L.off[B3C],
                     a->params + L.off[LOGSTD], a->actions, a->log_probs, a->advantages, a->returns, a->adv_stats, inv_mg, a->hp.clip_range,
-                    a->hp.critic_coef, a->hp.ratio_delta_metric != 0.f ? 1 : 0, dZ2, dhead, headpart, ws_ptr<float>(ws, P.off_dZ1)};
+                    a->hp.critic_coef, a->hp.ratio_delta_metric != 0.f ? 1 : 0, dZ2, dhead, headpart, h.ratio_abs, ws_ptr<float>(ws, P.off_dZ1)};
     const int rc = ppo_head_gemm_path(ha, st);
     if (rc) return rc;
+    record_train_head(4, 0, 0, 0);
     return 1;  // the path writes ONE partial block in the fused kernel's layout
   }
   if (!fast_head) {
     RLX_DISPATCH_NCH(KC_HEAD_TRAIN, head_flops, head_bytes, H, ppo_head_train_kernel, head_blocks, 256, smem, st, h);
+    const int nch = (int)ceil_div(H, 32);  // RLX_DISPATCH_NCH_B's buckets
+    record_train_head(0, nch <= 2 ? 2 : nch <= 4 ? 4 : nch <= 8 ? 8 : nch <= 16 ? 16 : 32, 0, bf16);
     return head_blocks;
   }
   HeadTrain2Extra ex{dh_ld};
@@ -433,6 +444,7 @@ static int launch_train_head(const rlx_ppo_minibatch_args* a, const PpoLayout& L
   do {                                                                                                                              \
     RLX_CHECK_CUDA(cudaFuncSetAttribute(ppo_head_train4_kernel<H_, NT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem4)); \
     RLX_LAUNCH_C(KC_HEAD_TRAIN, head_flops, head_bytes, (ppo_head_train4_kernel<H_, NT_>), head_blocks, 256, smem4, st, h, ex);     \
+    record_train_head(3, H_, NT_, 0);                                                                                               \
   } while (0)
 #define RLX_HEAD4_NT(H_)              \
   do {                                \
@@ -451,6 +463,7 @@ static int launch_train_head(const rlx_ppo_minibatch_args* a, const PpoLayout& L
   do {                                                                                                                                \
     RLX_CHECK_CUDA(cudaFuncSetAttribute(ppo_head_train3_kernel<H_, AM_, BF_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
     RLX_LAUNCH_C(KC_HEAD_TRAIN, head_flops, head_bytes, (ppo_head_train3_kernel<H_, AM_, BF_>), head_blocks, 256, smem, st, h, ex);    \
+    record_train_head(2, H_, AM_, BF_);                                                                                               \
   } while (0)
 #define RLX_HEAD3(H_, AM_)                          \
   do {                                              \
@@ -476,6 +489,7 @@ static int launch_train_head(const rlx_ppo_minibatch_args* a, const PpoLayout& L
   do {                                                                                                                                \
     RLX_CHECK_CUDA(cudaFuncSetAttribute(ppo_head_train2_kernel<NCH_, AM_, BF_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
     RLX_LAUNCH_C(KC_HEAD_TRAIN, head_flops, head_bytes, (ppo_head_train2_kernel<NCH_, AM_, BF_>), head_blocks, 256, smem, st, h, ex);  \
+    record_train_head(1, NCH_, AM_, BF_);                                                                                             \
   } while (0)
 #define RLX_HEAD2(NCH_, AM_)                        \
   do {                                              \
@@ -531,6 +545,7 @@ static int launch_head_wgrad(const PpoLayout& L, const TrainPlan& P, long long m
       RLX_CHECK_CUDA(cudaFuncSetAttribute(ppo_head_wgrad_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem));
       RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad_kernel<64>, wg, 256, wsmem, st, w);
     }
+    record_head_wgrad(0, A <= 8 ? 8 : A <= 32 ? 32 : 64);
     count_gemm_path(GP_HEAD_WGRAD_SIMT);
     w3 = chunked_w3(L, part3, wgrad_chunks);
     return RLX_OK;
@@ -548,6 +563,7 @@ static int launch_head_wgrad(const PpoLayout& L, const TrainPlan& P, long long m
     g3.bf16 = bf16;
     const int rc = tc_gemm(g3, false, false, TC_NONE, 2, KC_HEAD_WGRAD, m, m, st);
     if (rc == RLX_OK) {
+      record_head_wgrad(2, 0);
       // net 1 (critic half of H2), row `act` of its [dh_ld, H] block
       w3 = W3Partials{part3, S3.splits, 2LL * dh_ld * H, (long long)dh_ld * H + (long long)A * H};
       return RLX_OK;
@@ -558,13 +574,19 @@ static int launch_head_wgrad(const PpoLayout& L, const TrainPlan& P, long long m
   HeadWgrad2P w{(int)m, H, A, dh_ld, kHeadWgradRows, H2, dhead, part3};
   const unsigned wthreads = (unsigned)(ceil_div(H, 32) * 32);
   const size_t wsmem = (size_t)kHeadWgradRows * dh_ld * sizeof(float);
-  if (A + 1 <= 4) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<4>, wgrad_chunks, wthreads, wsmem, st, w);
-  else if (A + 1 <= 8) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<8>, wgrad_chunks, wthreads, wsmem, st, w);
-  else if (A + 1 <= 12) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<12>, wgrad_chunks, wthreads, wsmem, st, w);
-  else if (A + 1 <= 16) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<16>, wgrad_chunks, wthreads, wsmem, st, w);
-  else if (A + 1 <= 20) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<20>, wgrad_chunks, wthreads, wsmem, st, w);
-  else if (A + 1 <= 24) RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<24>, wgrad_chunks, wthreads, wsmem, st, w);
-  else RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<32>, wgrad_chunks, wthreads, wsmem, st, w);
+#define RLX_WGRAD3(AM_)                                                                                                 \
+  do {                                                                                                                  \
+    RLX_LAUNCH_C(KC_HEAD_WGRAD, wflops, wbytes, ppo_head_wgrad3_kernel<AM_>, wgrad_chunks, wthreads, wsmem, st, w);     \
+    record_head_wgrad(1, AM_);                                                                                          \
+  } while (0)
+  if (A + 1 <= 4) RLX_WGRAD3(4);
+  else if (A + 1 <= 8) RLX_WGRAD3(8);
+  else if (A + 1 <= 12) RLX_WGRAD3(12);
+  else if (A + 1 <= 16) RLX_WGRAD3(16);
+  else if (A + 1 <= 20) RLX_WGRAD3(20);
+  else if (A + 1 <= 24) RLX_WGRAD3(24);
+  else RLX_WGRAD3(32);
+#undef RLX_WGRAD3
   count_gemm_path(GP_HEAD_WGRAD_SIMT);
   w3 = chunked_w3(L, part3, wgrad_chunks);
   return RLX_OK;
@@ -678,6 +700,7 @@ static GradReduceP make_grad_reduce(const rlx_ppo_minibatch_args* a, const PpoLa
 // `fuse_norms`: the assembly kernel also leaves the two squared clip norms in the workspace (off_barrier + 16 bytes) and bumps Adam's
 // step counter, so that clip + Adam can follow without the separate sum-of-squares launch.
 static int minibatch_fwdbwd(const rlx_ppo_minibatch_args* a, void* stream, bool fuse_norms = false) {
+  for (int& v : g_head_path) v = -1;
   TrainPlan P;
   int rc = check_mb_args(a, true, P);
   if (rc) return rc;
@@ -913,6 +936,12 @@ extern "C" int rlx_debug_tf32_split_f32(const float* src, int64_t batch, int64_t
   RLX_CHECK_ARG(src && hi && lo && batch > 0 && rows > 0 && cols > 0 && batch * rows * cols < (1LL << 31), "bad arguments");
   const Tf32SplitJob job{src, hi, lo, (int)batch, (int)rows, (int)cols, trans ? 1 : 0};
   return tf32_split(&job, 1, KC_OTHER, (cudaStream_t)stream);
+}
+
+extern "C" int rlx_debug_ppo_head_path(int32_t* out) {
+  RLX_CHECK_ARG(out != nullptr, "out is null");
+  for (int i = 0; i < 6; ++i) out[i] = g_head_path[i];
+  return RLX_OK;
 }
 
 extern "C" int rlx_set_head_engine(int engine) {

@@ -25,7 +25,7 @@ __global__ void loss_rows_kernel(const float* __restrict__ Mean, const float* __
                                  const float* __restrict__ logp_old, const float* __restrict__ adv, const float* __restrict__ ret,
                                  const float* __restrict__ logstd, const float* __restrict__ adv_stats, long long m, int A, int dh_ld,
                                  float clip_range, float critic_coef, float inv_mg, int ratio_delta_metric, float* __restrict__ dhead,
-                                 float* __restrict__ dLs, float* __restrict__ terms) {
+                                 float* __restrict__ dLs, float* __restrict__ terms, float* __restrict__ ratio_abs) {
   const long long r = gtid();
   if (r >= m) return;
   float lp = 0.f;
@@ -56,6 +56,7 @@ __global__ void loss_rows_kernel(const float* __restrict__ Mean, const float* __
   terms[4 * r + 1] = 0.5f * verr * verr;
   terms[4 * r + 2] = (ratio - 1.f) - logratio;
   terms[4 * r + 3] = ratio_delta_metric ? fabsf(ratio - 1.f) : ((fabsf(ratio - 1.f) > clip_range) ? 1.f : 0.f);
+  if (ratio_abs != nullptr) ratio_abs[r] = fabsf(ratio - 1.f);
 }
 
 }  // namespace headgemm
@@ -82,7 +83,7 @@ int ppo_head_gemm_path(const HeadGemmArgs& a, cudaStream_t st) {
   HG_TRY((launch_sgemm<true, true, EPI_BIAS>(gv, 1, st, KC_GEMM_FWD)));
   // (2) per-row loss and head gradients
   RLX_FLAT_LAUNCH(loss_rows_kernel, m, st, Mean, V, a.actions, a.logp_old, a.adv, a.ret, a.logstd, a.adv_stats, m, A, dh, a.clip_range, a.critic_coef,
-                  a.inv_mg, a.ratio_delta_metric, a.dhead, dLs, terms);
+                  a.inv_mg, a.ratio_delta_metric, a.dhead, dLs, terms, a.ratio_abs);
   // (3) dZ2 = (dhead . W3) * (1 - H2^2): A k-major (dhead), B n-major (W3p[a, h] read as B[k = a][n = h]), tanh' epilogue on the matching half
   GemmP gp{};
   gp.A = a.dhead; gp.B = a.W3p; gp.C = a.dZ2; gp.aux = a.H2;
@@ -103,17 +104,27 @@ int ppo_head_gemm_path(const HeadGemmArgs& a, cudaStream_t st) {
 
 }  // namespace rlx
 
-// test / bring-up entry: the path on caller-provided buffers
+// test / bring-up entries: the path on caller-provided buffers.  The _ratio_ form also takes the optional per-row |ratio - 1| output
+// (ratio_abs); the original signature stays as it was for its existing callers and passes none.
 using namespace rlx;
+extern "C" int rlx_debug_ppo_head_gemm_ratio_f32(int64_t m, int32_t hidden, int32_t act_dim, const float* H2, const float* W3p, const float* W3c,
+                                                 const float* b3p, const float* b3c, const float* logstd, const float* actions, const float* logp_old,
+                                                 const float* adv, const float* ret, const float* adv_stats, float inv_mg, float clip_range,
+                                                 float critic_coef, int32_t ratio_delta_metric, float* dZ2, float* dhead, float* headpart,
+                                                 float* ratio_abs, float* scratch, void* stream) {
+  RLX_CHECK_ARG(m > 0 && hidden > 0 && act_dim > 0 && act_dim <= 64, "bad sizes");
+  RLX_CHECK_ARG(H2 && W3p && W3c && b3p && b3c && logstd && actions && logp_old && adv && ret && adv_stats && dZ2 && dhead && headpart && scratch,
+                "null pointer");
+  rlx::HeadGemmArgs a{m, hidden, act_dim, (int)(rlx::ceil_div(act_dim + 1, 4) * 4), H2, W3p, W3c, b3p, b3c, logstd, actions, logp_old, adv, ret,
+                      adv_stats, inv_mg, clip_range, critic_coef, ratio_delta_metric, dZ2, dhead, headpart, ratio_abs, scratch};
+  return rlx::ppo_head_gemm_path(a, (cudaStream_t)stream);
+}
+
 extern "C" int rlx_debug_ppo_head_gemm_f32(int64_t m, int32_t hidden, int32_t act_dim, const float* H2, const float* W3p, const float* W3c,
                                            const float* b3p, const float* b3c, const float* logstd, const float* actions, const float* logp_old,
                                            const float* adv, const float* ret, const float* adv_stats, float inv_mg, float clip_range,
                                            float critic_coef, int32_t ratio_delta_metric, float* dZ2, float* dhead, float* headpart, float* scratch,
                                            void* stream) {
-  RLX_CHECK_ARG(m > 0 && hidden > 0 && act_dim > 0 && act_dim <= 64, "bad sizes");
-  RLX_CHECK_ARG(H2 && W3p && W3c && b3p && b3c && logstd && actions && logp_old && adv && ret && adv_stats && dZ2 && dhead && headpart && scratch,
-                "null pointer");
-  rlx::HeadGemmArgs a{m, hidden, act_dim, (int)(rlx::ceil_div(act_dim + 1, 4) * 4), H2, W3p, W3c, b3p, b3c, logstd, actions, logp_old, adv, ret,
-                      adv_stats, inv_mg, clip_range, critic_coef, ratio_delta_metric, dZ2, dhead, headpart, scratch};
-  return rlx::ppo_head_gemm_path(a, (cudaStream_t)stream);
+  return rlx_debug_ppo_head_gemm_ratio_f32(m, hidden, act_dim, H2, W3p, W3c, b3p, b3c, logstd, actions, logp_old, adv, ret, adv_stats, inv_mg,
+                                           clip_range, critic_coef, ratio_delta_metric, dZ2, dhead, headpart, nullptr, scratch, stream);
 }

@@ -14,7 +14,8 @@ struct HeadGemmArgs {
   float* dZ2;             // [m, 2H] out
   float* dhead;           // [m, dh_ld] out: dMean | dV | zero padding
   float* headpart;        // [2A + 5 + 2H] out: db3p | db3c | dlogstd | pg | vl | kl | cf | db2p | db2c  (one block)
-  float* scratch;         // >= m * (2A + 8) + (m / 256 + 2) * max(2H, 8) floats
+  float* ratio_abs;       // optional [m] out: |ratio - 1| of every row (ESPO's delta_calc_operator = median), or null
+  float* scratch;        // >= m * (2A + 8) + (m / 256 + 2) * max(2H, 8) floats
 };
 
 // floats of `scratch` the path needs for m rows

@@ -93,14 +93,14 @@ def _hp(ent):
     return make_hparams(CLIP, ent, CRITIC_COEF, MAX_NORM)
 
 
-def _f64(d):
-    return {n: v.detach().to(DEV, torch.float64) for n, v in d.items()}
+def _f64(d, dev=DEV):
+    return {n: v.detach().to(dev, torch.float64) for n, v in d.items()}
 
 
 SUMMED_BIASES = ("policy_mean.4.bias", "critic.4.bias")
 
 
-def _oracle64(pol, cri, mb, ent):
+def _oracle64(pol, cri, mb, ent, dev=DEV):
     """oracle.Learner.grads in float64: (gradients as float64 numpy arrays by parameter name, the norm each is measured against, losses).
 
     The norm is ||g64||, except for the two last-layer biases: their gradients are sums of m signed per-row terms that largely cancel (the
@@ -112,11 +112,11 @@ def _oracle64(pol, cri, mb, ent):
     engines.  The terms are the gradients of row-wise copies of the bias ([m, out]; F.linear adds a
     bias broadcast to its output), which sum to the gradient itself."""
     m = mb["states"].shape[0]
-    pol64, cri64 = _f64(pol), _f64(cri)
+    pol64, cri64 = _f64(pol, dev), _f64(cri, dev)
     pol64["policy_mean.4.bias"] = pol64["policy_mean.4.bias"].expand(m, -1).clone()
     cri64["critic.4.bias"] = cri64["critic.4.bias"].expand(m, -1).clone()
     L = O.Learner(pol64, cri64, clip_range=CLIP, entropy_coef=ent, critic_coef=CRITIC_COEF)
-    gp, gc, met = L.grads(*(mb[n].to(DEV, torch.float64) for n in NAMES))
+    gp, gc, met = L.grads(*(mb[n].to(dev, torch.float64) for n in NAMES))
     g = {n: v.cpu().numpy() for n, v in {**gp, **gc}.items()}
     norms = {n: float(np.linalg.norm(v)) for n, v in g.items()}
     for n in SUMMED_BIASES:
@@ -134,7 +134,7 @@ def _named_grads(k, grads):
     return {n: v.numpy().astype(np.float64) for n, v in {**gpol, **gcri}.items()}
 
 
-def _minibatch_case(obs, act, hidden, m):
+def _minibatch_case(obs, act, hidden, m, dev=DEV):
     """Seeded parameters and minibatch as test_gpu_parity.py's test_minibatch_gradients_vs_oracle_autograd builds them: old log-probs near
     the policy's, so that the ratios straddle the clip range."""
     pol, cri = O.init_params(obs, act, hidden, std_dev=0.9, seed=m)
@@ -142,13 +142,13 @@ def _minibatch_case(obs, act, hidden, m):
     for w in list(pol.values()) + list(cri.values()):
         w.add_(0.02 * torch.randn(w.shape, generator=g))
     mb = _random_minibatch(obs, act, m, seed=m + 2)
-    mb["log_probs"] = _logp64(pol, mb) + 0.15 * torch.randn(m, generator=g)
+    mb["log_probs"] = _logp64(pol, mb, dev) + 0.15 * torch.randn(m, generator=g)
     return pol, cri, mb
 
 
-def _logp64(pol, mb):
+def _logp64(pol, mb, dev=DEV):
     with torch.no_grad():
-        lp, _ = O.get_logprob_entropy(_f64(pol), mb["states"].to(DEV, torch.float64), mb["actions"].to(DEV, torch.float64))
+        lp, _ = O.get_logprob_entropy(_f64(pol, dev), mb["states"].to(dev, torch.float64), mb["actions"].to(dev, torch.float64))
     return lp.float().cpu()
 
 

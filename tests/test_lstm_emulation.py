@@ -512,16 +512,18 @@ def test_emulated_nstep_replay_matches_reference_golden(tmp_path):
                 assert np.array_equal(got, ref), f"{tag}/{name} vs reference"
 
 
-@pytest.mark.parametrize("m,hid,act,rd", [(300, 16, 3, 0), (1000, 64, 17, 0), (257, 32, 6, 1)])
+@pytest.mark.parametrize("m,hid,act,rd", [(300, 16, 3, 0), (1000, 64, 17, 0), (257, 32, 6, 1), (129, 24, 5, 2)])
 def test_emulated_ppo_head_gemm_path(tmp_path, m, hid, act, rd):
     """rl_x_b200/csrc/ppo_head_gemm.cu (the opt-in GEMM formulation of the PPO loss head) compiled for the host, against autograd of the PPO
     loss (ppo.py:121-160) from the layer-2 activations: dZ2, the dW3 operand dhead, and the partial block (bias / log-std gradients,
-    metric sums) in the layout the rest of the update consumes."""
+    metric sums) in the layout the rest of the update consumes.  rd = 2 (ESPO's median operator) goes through the _ratio_ entry, which also
+    leaves |ratio - 1| per row, the values the update's median selects from."""
     out = tmp_path / "libheadgemm_emu.so"
     subprocess.run(emu_build_cmd(out, os.path.join(ROOT, "rl_x_b200", "csrc", "ppo_head_gemm.cu")), check=True)
     lib = C.CDLL(str(out))
     lib.rlx_debug_ppo_head_gemm_f32.argtypes = ([C.c_int64, C.c_int32, C.c_int32] + [C.c_void_p] * 11 + [C.c_float] * 3 + [C.c_int32] +
                                                 [C.c_void_p] * 5)
+    lib.rlx_debug_ppo_head_gemm_ratio_f32.argtypes = lib.rlx_debug_ppo_head_gemm_f32.argtypes + [C.c_void_p]
     torch.manual_seed(m)
     clip, cc = 0.2, 0.5
     Z2 = (torch.randn(m, 2 * hid) * 0.8).requires_grad_(True)
@@ -550,9 +552,18 @@ def test_emulated_ppo_head_gemm_path(tmp_path, m, hid, act, rd):
     dZ2, dhead, part = np.zeros((m, 2 * hid), np.float32), np.full((m, dh_ld), np.nan, np.float32), np.zeros(2 * act + 5 + 2 * hid, np.float32)
     scratch = np.zeros(m * (2 * act + 8) + (m // 256 + 2) * max(2 * hid, 8) + 64, np.float32)
     ins = [f(H2), f(W3p), f(W3c), f(b3p), f(b3c), f(logstd), f(actions), f(logp_old), f(adv), f(ret), f(stats)]
-    rc = lib.rlx_debug_ppo_head_gemm_f32(m, hid, act, *[x.ctypes.data for x in ins], 1.0 / m, clip, cc, rd, dZ2.ctypes.data, dhead.ctypes.data,
-                                         part.ctypes.data, scratch.ctypes.data, None)
+    rabs = np.full(m, np.nan, np.float32)
+    if rd == 2:
+        rc = lib.rlx_debug_ppo_head_gemm_ratio_f32(m, hid, act, *[x.ctypes.data for x in ins], 1.0 / m, clip, cc, rd, dZ2.ctypes.data,
+                                                   dhead.ctypes.data, part.ctypes.data, rabs.ctypes.data, scratch.ctypes.data, None)
+    else:
+        rc = lib.rlx_debug_ppo_head_gemm_f32(m, hid, act, *[x.ctypes.data for x in ins], 1.0 / m, clip, cc, rd, dZ2.ctypes.data, dhead.ctypes.data,
+                                             part.ctypes.data, scratch.ctypes.data, None)
     assert rc == 0
+    if rd == 2:
+        # fp32 ratios against autograd's fp32 ratios: a few ulps of the log-ratio, i.e. of the ratio itself, not of |ratio - 1|
+        r = ratio.detach().double().numpy()
+        assert np.all(np.abs(rabs - np.abs(r - 1)) <= 1e-5 * np.maximum(r, 1)), np.abs(rabs - np.abs(r - 1)).max()
     tol = dict(rtol=2e-4, atol=2e-7)
     np.testing.assert_allclose(dZ2, f(Z2.grad), **tol)
     np.testing.assert_allclose(dhead[:, :act], f(mean.grad), **tol)
